@@ -539,8 +539,8 @@ __global__ void __launch_bounds__(512, 1) k_fused_biquad(FusedArgs a, uint32_t n
 //   L  tile k+2 : each row's input window (<= TT*from/to + 3 frames) is fetched by the bulk-copy engine
 //                 (cp.async.bulk global -> shared, completion counted on an mbarrier), two tiles ahead,
 //                 so stage A never touches global memory and never waits for HBM latency.
-// 1024 threads, one loop per role: 23 stage-A warps (one row each, up to nine take a second row), the loader warp,
-// the recurrence warp alone on its SM sub-partition, stage C on two of the stage-A warps.
+// 1024 threads, one loop per role: 21 stage-A warps (one row each, up to eleven take a second row), the loader warp,
+// the recurrence warp alone on its SM sub-partition, stage C on two warps of the stage-A sub-partitions.
 // ---------------------------------------------------------------------------------------------------
 constexpr int NWIN = 3;                 // input-window ring (tile k .. k+2)
 constexpr int WSTRIDE = 320;            // floats per row window (>= 3 + TT*from/to + 3, multiple of 4): from/to <= 1.2
@@ -690,6 +690,56 @@ __device__ __forceinline__ void hot_issue_window(const FusedRow& r, const HotTil
 // Partial tiles (stream start / end, same-rate rows, the IEEE redo) take the strided path below: lane l works on
 // positions l + 32u, x goes through the row in shared memory, `row[-2C..-1]` are pad slots for the tail.
 // HASB = false (no filter in the chain: resample -> gains -> mix): the row receives x itself, there is no tail.
+// One interior sample: lerp of the taps (x0, x1) at numerator nfc with the exact-reciprocal division; `bad` collects
+// "operand outside the guarded range".
+template <bool NOGAIN>
+__device__ __forceinline__ float hot_lerp(float x0, float x1, float nfc, float den_f, float rcp_den, const float* pre, uint32_t n_pre,
+                                          const float* mid, uint32_t n_mid, bool& bad) {
+    const float a0 = gains<NOGAIN>(x0, pre, n_pre), a1 = gains<NOGAIN>(x1, pre, n_pre);
+    const float m = mul(sub(a1, a0), nfc);
+    const float q0 = mul(m, rcp_den);
+    const float q = __fmaf_rn(__fmaf_rn(-q0, den_f, m), rcp_den, q0);
+    // guarded range as one unsigned compare on the exponent field: 2^-100 <= |m| < 2^100; m == 0
+    // (also outside) yields q = m = +-0 exactly as the division would
+    const uint32_t e = __float_as_uint(m) & 0x7fffffffu;
+    const bool in_range = e - 0x0d800000u < 0x64000000u;
+#ifdef RB_HOT_TIMING
+    if (!(g_hot_skip & 32))               // ablation: no range check
+#endif
+    bad |= !in_range && e != 0u;
+    return gains<NOGAIN>(add(a0, in_range ? q : m), mid, n_mid);
+}
+// Interior tile, after the vote: the lane's P consecutive x values -> t (the feed-forward half; x itself without a filter)
+// -> two 16-byte stores at row[P*lane ..].  xtail takes the tile's last 2C x values.
+template <int C, bool HASB>
+__device__ __forceinline__ void hot_ff_store(float b0, float b1, float b2, const float (&xv)[TT / 32], float (&xtail)[2 * C],
+                                             uint32_t lane, float* __restrict__ row) {
+    constexpr int P = TT / 32;
+    float tv[P];
+    if constexpr (HASB) {
+        float pv[2 * C];
+#pragma unroll
+        for (int j = 0; j < 2 * C; j++) {
+            const float up = __shfl_up_sync(0xffffffffu, xv[P - 2 * C + j], 1);
+            pv[j] = lane == 0 ? xtail[j] : up;
+        }
+#pragma unroll
+        for (int j = 0; j < 2 * C; j++) xtail[j] = __shfl_sync(0xffffffffu, xv[P - 2 * C + j], 31);
+#pragma unroll
+        for (int u = 0; u < P; u++) {
+            const float xm1 = u >= C ? xv[u >= C ? u - C : 0] : pv[C + u < 2 * C ? C + u : 0];
+            const float xm2 = u >= 2 * C ? xv[u >= 2 * C ? u - 2 * C : 0] : pv[u < 2 * C ? u : 0];
+            tv[u] = biquad_ff(b0, b1, b2, xv[u], xm1, xm2);
+        }
+    } else {
+#pragma unroll
+        for (int u = 0; u < P; u++) tv[u] = xv[u];
+    }
+    float4* o = reinterpret_cast<float4*>(row + P * lane);
+#pragma unroll
+    for (int u = 0; u < P; u += 4) o[u / 4] = make_float4(tv[u], tv[u + 1], tv[u + 2], tv[u + 3]);
+}
+
 template <bool NOGAIN, int C, bool HASB>
 __device__ __forceinline__ void hot_stage_a(const FusedRow& r, const HotTile& ht, uint32_t n_pre, uint32_t n_mid,
                                             uint32_t lane, uint32_t lane_q, uint32_t lane_r, float (&xtail)[2 * C],
@@ -729,46 +779,10 @@ __device__ __forceinline__ void hot_stage_a(const FusedRow& r, const HotTile& ht
                 w += step_w;
                 if (nf >= den_f) nf = sub(nf, den_f), w += C;
 #pragma unroll
-                for (int c = 0; c < C; c++) {
-                    const float a0 = gains<NOGAIN>(x0[c], pre, n_pre), a1 = gains<NOGAIN>(x1[c], pre, n_pre);
-                    const float m = mul(sub(a1, a0), nfc);
-                    const float q0 = mul(m, rcp_den);
-                    const float q = __fmaf_rn(__fmaf_rn(-q0, den_f, m), rcp_den, q0);
-                    // guarded range as one unsigned compare on the exponent field: 2^-100 <= |m| < 2^100; m == 0
-                    // (also outside) yields q = m = +-0 exactly as the division would
-                    const uint32_t e = __float_as_uint(m) & 0x7fffffffu;
-                    const bool in_range = e - 0x0d800000u < 0x64000000u;
-#ifdef RB_HOT_TIMING
-                    if (!(g_hot_skip & 32))               // ablation: no range check
-#endif
-                    bad |= !in_range && e != 0u;
-                    xv[f * C + c] = gains<NOGAIN>(add(a0, in_range ? q : m), mid, n_mid);
-                }
+                for (int c = 0; c < C; c++) xv[f * C + c] = hot_lerp<NOGAIN>(x0[c], x1[c], nfc, den_f, rcp_den, pre, n_pre, mid, n_mid, bad);
             }
             if (!__any_sync(0xffffffffu, bad)) {
-                float tv[P];
-                if constexpr (HASB) {
-                    float pv[2 * C];
-#pragma unroll
-                    for (int j = 0; j < 2 * C; j++) {
-                        const float up = __shfl_up_sync(0xffffffffu, xv[P - 2 * C + j], 1);
-                        pv[j] = lane == 0 ? xtail[j] : up;
-                    }
-#pragma unroll
-                    for (int j = 0; j < 2 * C; j++) xtail[j] = __shfl_sync(0xffffffffu, xv[P - 2 * C + j], 31);
-#pragma unroll
-                    for (int u = 0; u < P; u++) {
-                        const float xm1 = u >= C ? xv[u >= C ? u - C : 0] : pv[C + u < 2 * C ? C + u : 0];
-                        const float xm2 = u >= 2 * C ? xv[u >= 2 * C ? u - 2 * C : 0] : pv[u < 2 * C ? u : 0];
-                        tv[u] = biquad_ff(b0, b1, b2, xv[u], xm1, xm2);
-                    }
-                } else {
-#pragma unroll
-                    for (int u = 0; u < P; u++) tv[u] = xv[u];
-                }
-                float4* o = reinterpret_cast<float4*>(row + P * lane);
-#pragma unroll
-                for (int u = 0; u < P; u += 4) o[u / 4] = make_float4(tv[u], tv[u + 1], tv[u + 2], tv[u + 3]);
+                hot_ff_store<C, HASB>(b0, b1, b2, xv, xtail, lane, row);
                 done = true;
             }
             // else: some operand was denormal / huge / NaN: redo this row-tile with IEEE divisions
@@ -818,19 +832,63 @@ __device__ __forceinline__ void hot_stage_a(const FusedRow& r, const HotTile& ht
         if (lane + 32u * (uint32_t)u < n) out[32 * u] = biquad_ff(b0, b1, b2, xv[u], xm1[u], xm2[u]);
 }
 
+// Stage A for the two mono rows of one warp when their tiles are in phase: both interior, the same rate pair (hence the same
+// lane constants) and the same r0.  Numerator and window offset then advance identically for both rows, so ONE index walk
+// (FADD, FSETP, the predicated adds, the address) serves both windows, and one vote covers both.  The two rows' loads and
+// arithmetic interleave; each row keeps its own window, gains, taps and tail.  Returns false when the vote fails: the caller
+// then runs each row on its own, which redoes the tile with IEEE divisions.
+template <bool NOGAIN, bool HASB>
+__device__ __forceinline__ bool hot_stage_a_pair(const FusedRow& ra, const FusedRow& rb, const HotTile& ha, const HotTile& hb,
+                                                 uint32_t n_pre, uint32_t n_mid, uint32_t lane, uint32_t lane_q, uint32_t lane_r,
+                                                 float (&tail_a)[2], float (&tail_b)[2], const float* win_a, const float* win_b,
+                                                 float* row_a, float* row_b) {
+    constexpr int P = TT / 32;
+    const uint32_t to = ra.uni.to;
+    const float den_f = ra.den_f, rcp_den = ra.rcp_den;
+    uint32_t num = ha.r0 + lane_r;
+    uint32_t di = lane_q;
+    if (num >= to) num -= to, di += 1;
+    const float* w = win_a + ha.woff + di;
+    const int db = (int)((win_b + hb.woff) - (win_a + ha.woff));   // row b's taps relative to row a's (warp-uniform)
+    const uint32_t step_w = ra.q32;
+    const float r1f = __uint2float_rn(ra.r32);
+    float nf = __uint2float_rn(num);
+    bool bad = false;
+    float xa[P], xb[P];
+#pragma unroll
+    for (int f = 0; f < P; f++) {
+        const float a0 = w[0], a1 = w[1], b0 = w[db], b1 = w[db + 1];
+        const float nfc = nf;
+        nf = add(nf, r1f);
+        w += step_w;
+        if (nf >= den_f) nf = sub(nf, den_f), w += 1;
+        xa[f] = hot_lerp<NOGAIN>(a0, a1, nfc, den_f, rcp_den, ra.pre, n_pre, ra.mid, n_mid, bad);
+        xb[f] = hot_lerp<NOGAIN>(b0, b1, nfc, den_f, rcp_den, rb.pre, n_pre, rb.mid, n_mid, bad);
+    }
+    if (__any_sync(0xffffffffu, bad)) return false;
+    hot_ff_store<1, HASB>(ra.b0, ra.b1, ra.b2, xa, tail_a, lane, row_a);
+    hot_ff_store<1, HASB>(rb.b0, rb.b1, rb.b2, xb, tail_b, lane, row_b);
+    return true;
+}
+
 // Warp roles (32 warps; sub-partition = warp % 4).  Measured: the recurrence warp must have its sub-partition
 // to itself.  Its dependent chain (FMUL -> FFMA -> FFMA, 12.9 cycles per sample when alone) needs every issue slot
 // on time: with the loader as its neighbour it ran at 16.4 cycles per sample, with stage-A warps at twice that.
 //   warp 31                  recurrence (stage B), alone on sub-partition 3 (warps 3,7,..,27 idle)
 //   warp 30                  loader (stage L, lane = row)
-//   the other 23 warps with warp % 4 != 3: stage A, slot = (warp/4)*3 + warp%4 owns row `slot`; rows 23..31 are the
-//   second rows of slots {0,3,9 | 1,4,10 | 2,5,8} and stage C runs on slots {6, 7}: the three sub-partitions carry about
-//   equal instruction counts (the loader sits where one row fewer does).
+//   the other 23 warps with warp % 4 != 3: stage A, slot = (warp/4)*3 + warp%4 (sub-partition = slot % 3).
+//   Default launch: stage C runs on slots {6, 7} (sub-partitions 0 and 1), which own no row.  The other 21 slots own
+//   rows 0..20 in slot order, and rows 21..31 are the second rows of slots {0,3,9,12 | 1,4,10,13 | 2,5,8}, taken in the
+//   order 0,1,2,3,4,5,9,10,8,12,13: sub-partitions 0 and 1 carry 11 rows and half of stage C each, sub-partition 2
+//   carries 10 rows and the loader.  A warp with two mono rows walks both in one pass when their tiles are in phase
+//   (hot_stage_a_pair), so a second row costs less than a first.
+//   Chain mode: stage C runs on warps 3 and 7 (below), all 23 slots own rows 0..22, and rows 23..31 are the second rows of
+//   slots {0,3,9 | 1,4,10 | 2,5,8} in the same order: 11, 11 and 10 rows + loader.
 // 32 rows need the narrow window stride (WSTRIDE_NARROW) to fit in shared memory; with the wide one a CTA takes 28.  On the
 // 132 SMs of an H100, 32 rows put the 4096 streams of the benchmarked batch into ONE wave of 128 CTAs (28 rows: 147 CTAs,
 // two waves, each walking the whole recurrence).
-constexpr uint32_t HOT_MAX_ROWS = 28;          // 23 slots + 5 second rows (wide windows)
-constexpr uint32_t HOT_MAX_ROWS_NARROW = 32;   // 23 slots + 9 second rows (mono, narrow windows)
+constexpr uint32_t HOT_MAX_ROWS = 28;          // 21 slots + 7 second rows (wide windows)
+constexpr uint32_t HOT_MAX_ROWS_NARROW = 32;   // 21 slots + 11 second rows (mono, narrow windows)
 constexpr uint32_t HOT_MAX_ROWS_STEREO = 28;   // 56 chains: a second recurrence warp (27, same sub-partition) takes rows 16..27
 constexpr uint32_t HOT_REC_WARP2 = 27;
 constexpr uint32_t HOT_REC_WARP = 31, HOT_LOAD_WARP = 30;
@@ -838,10 +896,17 @@ __device__ __forceinline__ int hot_row_slot(uint32_t warp) {
     if ((warp & 3u) == 3u || warp == HOT_LOAD_WARP) return -1;
     return (int)((warp >> 2) * 3u + (warp & 3u));   // 0..22
 }
-// second row of a slot (rows beyond the 23 slots), or -1
+// first row of a slot, or -1 (the stage-C slots of the default launch)
+template <bool CHAIN>
+__device__ __forceinline__ int hot_first_row(int slot) {
+    return CHAIN || slot < 6 ? slot : slot < 8 ? -1 : slot - 2;
+}
+// second row of a slot (rows beyond the slots' first rows), or -1
+template <bool CHAIN>
 __device__ __forceinline__ int hot_second_row(int slot) {
-    return slot == 0 ? 23 : slot == 3 ? 24 : slot == 1 ? 25 : slot == 2 ? 26 : slot == 5 ? 27
-         : slot == 9 ? 28 : slot == 4 ? 29 : slot == 10 ? 30 : slot == 8 ? 31 : -1;
+    constexpr int base = CHAIN ? 23 : 21;
+    const int j = slot < 6 ? slot : slot == 9 ? 6 : slot == 10 ? 7 : slot == 8 ? 8 : slot == 12 ? 9 : slot == 13 ? 10 : -1;
+    return j < 0 || base + j >= (int)HOT_MAX_ROWS_NARROW ? -1 : base + j;
 }
 // Stage C of the HOT kernel: one thread sums FOUR consecutive tile positions over the CTA's rows (row order =
 // the mixer's insertion order), 16-byte loads of y, the post-gain applied on the fly.  64 threads cover a tile.
@@ -988,6 +1053,10 @@ __global__ void __launch_bounds__(1024, 1) k_fused_hot(FusedArgs a) {
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const bool is_rec = warp == HOT_REC_WARP || (C == 2 && warp == HOT_REC_WARP2), is_loader = warp == HOT_LOAD_WARP;
     const int slot = hot_row_slot(warp);
+    // stage C: two warps of their own, 4 positions per thread, so that its loop state is never live beside a row's stage A.
+    // Default launch: slots 6 and 7 (sub-partitions 0 and 1).  Chain mode: warps 3 and 7 (idle otherwise; the recurrence warp's
+    // sub-partition has issue slots to spare) -- the hand-over is latency, not work, and must not sit behind a row's stage A.
+    const int mix_block = CHAIN ? (warp == 3 ? 0 : warp == 7 ? 1 : -1) : (slot == 6 ? 0 : slot == 7 ? 1 : -1);
     const bool nogain = a.n_pre == 0 && a.n_mid == 0;
     // prologue: the loader warp (lane = row) fetches the windows of tiles 0 and 1
     if (is_loader && lane < G) {
@@ -1125,76 +1194,8 @@ __global__ void __launch_bounds__(1024, 1) k_fused_hot(FusedArgs a) {
             HOT_BAR();
         }
 #undef FB
-    } else if (slot >= 0) {
-        // ---- stage A on tile it, stage C on tile it-2 ----
-        const bool has_first = (uint32_t)slot < G;
-        const int second = hot_second_row(slot);
-        const bool has_second = second >= 0 && (uint32_t)second < G;
-        // stage C: two warps, 4 positions per thread (slots without a second row, on different sub-partitions)
-        // (chain mode: stage C moves to two warps of its own, below -- the hand-over is latency, not work, and must not sit behind a row's stage A)
-        const int mix_block = CHAIN ? -1 : slot == 6 ? 0 : slot == 7 ? 1 : -1;
-        // (lane's first frame * from) divmod to for the rows this warp owns
-        uint32_t lane_q0 = 0, lane_r0 = 0, lane_q1 = 0, lane_r1 = 0;
-        if (has_first) {
-            const uint32_t p = lane * (uint32_t)(TT / 32 / C) * s_rows[slot].uni.from;
-            lane_q0 = p / s_rows[slot].uni.to;
-            lane_r0 = p - lane_q0 * s_rows[slot].uni.to;
-        }
-        if (has_second) {
-            const uint32_t p = lane * (uint32_t)(TT / 32 / C) * s_rows[second].uni.from;
-            lane_q1 = p / s_rows[second].uni.to;
-            lane_r1 = p - lane_q1 * s_rows[second].uni.to;
-        }
-        float xtail0[2 * C], xtail1[2 * C];   // x at the last two frames of the previous tile, per owned row
-#pragma unroll
-        for (int j = 0; j < 2 * C; j++) xtail0[j] = xtail1[j] = 0.f;
-        const FusedRow& rowA = s_rows[has_first ? slot : 0];
-        const FusedRow& rowB = s_rows[has_second ? second : 0];
-        uint32_t kw = 0, kb = 0, kh = 0, phase = 0;   // tile it
-        uint32_t cb = 0, ch = 0;                      // tile it-2
-        const uint32_t mix_t = ((uint32_t)(mix_block < 0 ? 0 : mix_block) * 32 + lane) * 4;
-        for (uint32_t it = 0; it < n_iter; it++) {
-            if (it < n_tiles) {
-                if (has_first && !HOT_SKIP(1)) {
-                    HOT_MBAR_WAIT(&s_full[kw], phase);
-                    float* tile = tiles + kb * tile_sz + HOT_PAD;
-                    const float* win = wins + kw * win_sz;
-                    {
-                        const HotTile& ht = s_ht[kh][slot];
-                        if (ht.lo < ht.hi) {
-                            if (nogain) hot_stage_a<true, C, HASB>(rowA, ht, a.n_pre, a.n_mid, lane, lane_q0, lane_r0, xtail0, win + slot * wstride, tile + slot * ROW_STRIDE);
-                            else hot_stage_a<false, C, HASB>(rowA, ht, a.n_pre, a.n_mid, lane, lane_q0, lane_r0, xtail0, win + slot * wstride, tile + slot * ROW_STRIDE);
-                        }
-                    }
-                    if (has_second && !HOT_SKIP(8)) {
-                        const HotTile& ht = s_ht[kh][second];
-                        if (ht.lo < ht.hi) {
-                            if (nogain) hot_stage_a<true, C, HASB>(rowB, ht, a.n_pre, a.n_mid, lane, lane_q1, lane_r1, xtail1, win + second * wstride, tile + second * ROW_STRIDE);
-                            else hot_stage_a<false, C, HASB>(rowB, ht, a.n_pre, a.n_mid, lane, lane_q1, lane_r1, xtail1, win + second * wstride, tile + second * ROW_STRIDE);
-                        }
-                    }
-                }
-                kw = kw + 1 == NWIN ? 0 : kw + 1;
-                phase ^= kw == 0;
-                kb = kb + 1 == NBUF ? 0 : kb + 1;
-                kh = kh + 1 == NHT ? 0 : kh + 1;
-            }
-            if (it >= 2) {
-                // ---- stage C ----
-                if (mix_block >= 0 && !HOT_SKIP(4)) {
-                    const uint64_t m0 = m_begin + (uint64_t)(it - 2) * TT;
-                    const bool full = m0 >= f_lo && m0 + TT <= f_hi;
-                    hot_mix4(tiles + cb * tile_sz + HOT_PAD, s_ht[ch], s_rows, G, a.n_post, mix_t, full, m0, a.mix_len, partial);
-                }
-                cb = cb + 1 == NBUF ? 0 : cb + 1;
-                ch = ch + 1 == NHT ? 0 : ch + 1;
-            }
-            HOT_BAR();
-        }
-    } else if (CHAIN && (warp == 3 || warp == 7)) {
-        // ---- chain mode, stage C on tile it-2: warps 3 and 7 (idle otherwise; the recurrence warp's sub-partition has issue slots to
-        // spare) wait for the CTA in front, add this CTA's rows to its running sum and hand it on ----
-        const int mix_block = warp == 3 ? 0 : 1;
+    } else if (mix_block >= 0) {
+        // ---- stage C on tile it-2 (chain mode: wait for the CTA in front, add this CTA's rows to its running sum, hand it on) ----
         const uint32_t mix_t = ((uint32_t)mix_block * 32 + lane) * 4;
         uint32_t cb = 0, ch = 0;
         for (uint32_t it = 0; it < n_iter; it++) {
@@ -1202,11 +1203,74 @@ __global__ void __launch_bounds__(1024, 1) k_fused_hot(FusedArgs a) {
                 if (!HOT_SKIP(4)) {
                     const uint64_t m0 = m_begin + (uint64_t)(it - 2) * TT;
                     const bool full = m0 >= f_lo && m0 + TT <= f_hi;
-                    hot_mix4(tiles + cb * tile_sz + HOT_PAD, s_ht[ch], s_rows, G, a.n_post, mix_t, full, m0, a.mix_len, partial, true, carry_row,
+                    hot_mix4(tiles + cb * tile_sz + HOT_PAD, s_ht[ch], s_rows, G, a.n_post, mix_t, full, m0, a.mix_len, partial, CHAIN, carry_row,
                              tagged_row, a.epoch * (n_iter + 1u) + (it - 2) + 1u);
                 }
                 cb = cb + 1 == NBUF ? 0 : cb + 1;
                 ch = ch + 1 == NHT ? 0 : ch + 1;
+            }
+            HOT_BAR();
+        }
+    } else if (slot >= 0) {
+        // ---- stage A on tile it ----
+        const int first = hot_first_row<CHAIN>(slot), second = hot_second_row<CHAIN>(slot);
+        const bool has_first = first >= 0 && (uint32_t)first < G;
+        const bool has_second = second >= 0 && (uint32_t)second < G;
+        const FusedRow& rowA = s_rows[has_first ? first : 0];
+        const FusedRow& rowB = s_rows[has_second ? second : 0];
+        // (lane's first frame * from) divmod to: shared by both rows when they have the same rate pair
+        const bool same_rate = rowA.uni.from == rowB.uni.from && rowA.uni.to == rowB.uni.to;
+        uint32_t lane_q = 0, lane_r = 0;
+        if (has_first) {
+            const uint32_t p = lane * (uint32_t)(TT / 32 / C) * rowA.uni.from;
+            lane_q = p / rowA.uni.to;
+            lane_r = p - lane_q * rowA.uni.to;
+        }
+        float xtail0[2 * C], xtail1[2 * C];   // x at the last two frames of the previous tile, per owned row
+#pragma unroll
+        for (int j = 0; j < 2 * C; j++) xtail0[j] = xtail1[j] = 0.f;
+        uint32_t kw = 0, kb = 0, kh = 0, phase = 0;   // tile it
+        for (uint32_t it = 0; it < n_iter; it++) {
+            if (it < n_tiles) {
+                if (has_first && !HOT_SKIP(1)) {
+                    HOT_MBAR_WAIT(&s_full[kw], phase);
+                    float* tile = tiles + kb * tile_sz + HOT_PAD;
+                    const float* win = wins + kw * win_sz;
+                    const int b = has_second ? second : first;
+                    const HotTile& ha = s_ht[kh][first];
+                    const HotTile& hb = s_ht[kh][b];
+                    const bool do_second = has_second && !HOT_SKIP(8);
+                    const float* win_a = win + first * wstride;
+                    const float* win_b = win + b * wstride;
+                    float* row_a = tile + first * ROW_STRIDE;
+                    float* row_b = tile + b * ROW_STRIDE;
+                    bool solo = true;
+                    if constexpr (C == 1) {
+                        if (do_second && same_rate && ha.interior && hb.interior && ha.r0 == hb.r0)   // warp-uniform
+                            solo = !(nogain ? hot_stage_a_pair<true, HASB>(rowA, rowB, ha, hb, a.n_pre, a.n_mid, lane, lane_q, lane_r, xtail0, xtail1, win_a, win_b, row_a, row_b)
+                                            : hot_stage_a_pair<false, HASB>(rowA, rowB, ha, hb, a.n_pre, a.n_mid, lane, lane_q, lane_r, xtail0, xtail1, win_a, win_b, row_a, row_b));
+                    }
+                    if (solo) {
+                        if (ha.lo < ha.hi) {
+                            if (nogain) hot_stage_a<true, C, HASB>(rowA, ha, a.n_pre, a.n_mid, lane, lane_q, lane_r, xtail0, win_a, row_a);
+                            else hot_stage_a<false, C, HASB>(rowA, ha, a.n_pre, a.n_mid, lane, lane_q, lane_r, xtail0, win_a, row_a);
+                        }
+                        if (do_second && hb.lo < hb.hi) {
+                            uint32_t qb = lane_q, rb = lane_r;
+                            if (!same_rate) {
+                                const uint32_t p = lane * (uint32_t)(TT / 32 / C) * rowB.uni.from;
+                                qb = p / rowB.uni.to;
+                                rb = p - qb * rowB.uni.to;
+                            }
+                            if (nogain) hot_stage_a<true, C, HASB>(rowB, hb, a.n_pre, a.n_mid, lane, qb, rb, xtail1, win_b, row_b);
+                            else hot_stage_a<false, C, HASB>(rowB, hb, a.n_pre, a.n_mid, lane, qb, rb, xtail1, win_b, row_b);
+                        }
+                    }
+                }
+                kw = kw + 1 == NWIN ? 0 : kw + 1;
+                phase ^= kw == 0;
+                kb = kb + 1 == NBUF ? 0 : kb + 1;
+                kh = kh + 1 == NHT ? 0 : kh + 1;
             }
             HOT_BAR();
         }

@@ -58,11 +58,12 @@ def main():
             ms = e0.elapsed_time(e1)
             what = " + ".join(v for k, v in names.items() if skip & k) or "full kernel"
             print(json.dumps({"streams": S, "channels": ch, "ms": round(ms, 4), "variant": what}))
-            # warp roles of k_fused_hot (rb_fused.cu: hot_row_slot / hot_second_row / stage C on slots 6, 7)
-            groups = {"two rows (w0,1,2,4,6)": [0, 1, 2, 4, 6], "row + stage C (w8,9)": [8, 9],
-                      "one row": [5, 10, 12, 13, 14, 16, 17, 18, 20, 21, 22, 24, 25, 26, 28, 29], "loader": [30],
+            # warp roles of k_fused_hot at 32 rows per CTA (rb_fused.cu: hot_row_slot / hot_first_row / hot_second_row, stage C
+            # on slots 6, 7); with fewer rows per CTA the later warps of a group own fewer rows or none
+            groups = {"two rows (w0,1,2,4,5,6,10,12,13,16,17)": [0, 1, 2, 4, 5, 6, 10, 12, 13, 16, 17], "stage C (w8,9)": [8, 9],
+                      "one row": [14, 18, 20, 21, 22, 24, 25, 26, 28, 29], "loader": [30],
                       "recurrence": [31] + ([27] if ch == 2 else [])}
-            n_cta = (S + 27) // 28 if ch == 1 else (S + 15) // 16
+            n_cta = int(b.mix_group and (S + b.mix_group - 1) // b.mix_group) or 1
             for g, ws in groups.items():
                 work = sum(buf[4 * w] for w in ws) / len(ws) / n_cta
                 bar = sum(buf[4 * w + 1] for w in ws) / len(ws) / n_cta
