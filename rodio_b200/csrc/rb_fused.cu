@@ -604,6 +604,19 @@ __device__ __forceinline__ void hot_timing_fence() {
 #define HOT_BAR() cta_bar()
 #define HOT_TIMING_END
 #endif
+// Stage-A outcomes, counted in row-tiles by the instrumented build -DRB_HOT_PATHS (tests/test_hot_rows_gpu.py), so that a test can
+// tell which paths of stage A it ran.  A row-tile ends in exactly one of PAIR, SOLO, REDO and STRIDED; PAIR_FAILED counts the
+// row-tiles of a failed pair vote, which then run solo and are counted again there.
+enum { HOT_PATH_PAIR = 0, HOT_PATH_PAIR_FAILED, HOT_PATH_SOLO, HOT_PATH_REDO, HOT_PATH_STRIDED, HOT_PATH_N = 8 };
+#ifdef RB_HOT_PATHS
+__device__ unsigned long long g_hot_paths[HOT_PATH_N];
+#define HOT_PATH(k_, n_)                                                                     \
+    do {                                                                                     \
+        if ((threadIdx.x & 31) == 0) atomicAdd(&g_hot_paths[k_], (unsigned long long)(n_)); \
+    } while (0)
+#else
+#define HOT_PATH(k_, n_) do { } while (0)
+#endif
 
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     asm volatile(
@@ -786,6 +799,9 @@ __device__ __forceinline__ void hot_stage_a(const FusedRow& r, const HotTile& ht
                 done = true;
             }
             // else: some operand was denormal / huge / NaN: redo this row-tile with IEEE divisions
+            HOT_PATH(done ? HOT_PATH_SOLO : HOT_PATH_REDO, 1);
+        } else {
+            HOT_PATH(HOT_PATH_STRIDED, 1);
         }
     }
     if (done) return;
@@ -1246,9 +1262,11 @@ __global__ void __launch_bounds__(1024, 1) k_fused_hot(FusedArgs a) {
                     float* row_b = tile + b * ROW_STRIDE;
                     bool solo = true;
                     if constexpr (C == 1) {
-                        if (do_second && same_rate && ha.interior && hb.interior && ha.r0 == hb.r0)   // warp-uniform
+                        if (do_second && same_rate && ha.interior && hb.interior && ha.r0 == hb.r0) {   // warp-uniform
                             solo = !(nogain ? hot_stage_a_pair<true, HASB>(rowA, rowB, ha, hb, a.n_pre, a.n_mid, lane, lane_q, lane_r, xtail0, xtail1, win_a, win_b, row_a, row_b)
                                             : hot_stage_a_pair<false, HASB>(rowA, rowB, ha, hb, a.n_pre, a.n_mid, lane, lane_q, lane_r, xtail0, xtail1, win_a, win_b, row_a, row_b));
+                            HOT_PATH(solo ? HOT_PATH_PAIR_FAILED : HOT_PATH_PAIR, 2);
+                        }
                     }
                     if (solo) {
                         if (ha.lo < ha.hi) {
@@ -1580,6 +1598,17 @@ extern "C" int rb_debug_hot_timing(unsigned long long* out, int reset) {
     if (e == cudaSuccess && reset) {
         unsigned long long z[128] = {0};
         e = cudaMemcpyToSymbol(g_hot_timing, z, sizeof(z));
+    }
+    return (int)e;
+}
+#endif
+#ifdef RB_HOT_PATHS
+// out[HOT_PATH_*]: k_fused_hot's row-tiles per stage-A outcome since the last reset (8 counters, 5 in use)
+extern "C" int rb_debug_hot_paths(unsigned long long* out, int reset) {
+    cudaError_t e = cudaMemcpyFromSymbol(out, g_hot_paths, sizeof(unsigned long long) * HOT_PATH_N);
+    if (e == cudaSuccess && reset) {
+        unsigned long long z[HOT_PATH_N] = {0};
+        e = cudaMemcpyToSymbol(g_hot_paths, z, sizeof(z));
     }
     return (int)e;
 }
