@@ -284,6 +284,21 @@ rb_status rb_stream_plan(const rb_stream_desc* desc, uint16_t mixer_channels, ui
 rb_status rb_streams_plan(const rb_stream_desc* descs, size_t n_streams, size_t stream, uint16_t mixer_channels, uint32_t mixer_sample_rate,
                           uint64_t* out_len, uint16_t* chain_channels, uint32_t* chain_rate, uint64_t* chain_len);
 
+/* Adapters on the MixerSource itself, in array order: [AMPLIFY] [LIMIT] [AMPLIFY] (each optional, >= 1 effect).
+ * rodio: mixer_source.amplify(a).limit(settings).amplify(b) (src/mixer.rs:70-136, src/source/limit.rs).  n_effects = 0 removes it.
+ * Records as for a source: RB_FX_AMPLIFY f32[0]; RB_FX_LIMIT f32[0..1], ns[0..1], its coefficients for the mixer's rate and
+ * channel count (the mixer's format never changes).  The chain runs over the active runs of the mix as ONE sequence: where
+ * MixerSource::next() returns None (no source playing, a later Mixer::add still scheduled) the chain is not pulled, the
+ * sample stays 0.0 and the limiter keeps its state.  Every call that hands out the mix (rb_batch_render_mix(_device),
+ * rb_batch_mix_device_ptr, rb_batch_read_mix, rb_session_render) then returns the mastered mix; rb_batch_kernel_family and
+ * rb_batch_mix_group still describe the sum, rb_batch_launches_per_render counts one launch more (k_master).
+ * RB_ERR_UNSUPPORTED: another kind, another order, a second LIMIT or two AMPLIFYs on one side of it.
+ * rb_batch_set_master: RB_ERR_UNALIGNED_FRAMES when an active run of the mix ends inside a frame (a chain with a trailing
+ * partial frame); rb_batch_render_mix_allreduce refuses a batch with a master chain (RB_ERR_UNSUPPORTED).
+ * rb_session_set_master: before the first rendered frame (RB_ERR_STATE after it); the limiter state carries from block to
+ * block and travels in the state blob, which only a session with the same master chain accepts. */
+rb_status rb_batch_set_master(rb_batch* b, const rb_effect* effects, uint32_t n_effects);
+
 /* Drain the MixerSource (src/mixer.rs:120-136) for the whole batch.
  *   _device: enqueue only; result stays in HBM (rb_batch_mix_device_ptr), no sync.
  *   host   : enqueue, copy `min(mix_len, max_samples)` samples to out_host, sync. */
@@ -327,6 +342,8 @@ typedef struct rb_session rb_session;
 rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels, uint32_t mixer_sample_rate, const rb_stream_desc* descs,
                             size_t n_streams, uint32_t fifo_frames, uint32_t max_block_frames, rb_session** out);
 rb_status rb_session_destroy(rb_session* s);
+/* mixer_source.amplify(a).limit(settings).amplify(b) on the session's output: see rb_batch_set_master. */
+rb_status rb_session_set_master(rb_session* s, const rb_effect* effects, uint32_t n_effects);
 /* n_frames more frames of source `stream` have arrived; end_of_stream != 0: the source's Iterator::next would return
  * None after them.  RB_ERR_BUFFER_TOO_SMALL when its FIFO cannot take them (render first). */
 rb_status rb_session_push(rb_session* s, size_t stream, const float* pcm, uint64_t n_frames, int end_of_stream);

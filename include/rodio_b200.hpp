@@ -7,6 +7,7 @@
 #pragma once
 #include <chrono>
 #include <cstdint>
+#include <cstring>
 #include <memory>
 #include <optional>
 #include <stdexcept>
@@ -265,6 +266,7 @@ struct Shared {
     bool dirty = true;
     std::vector<Sample> rendered;
     std::vector<uint8_t> active;       // position has at least one source playing
+    std::vector<rb_effect> rendered_master;   // the MixerSource adapters `rendered` went through
 };
 
 // mixer::Mixer — src/mixer.rs:47-66 ; add is infallible like the reference
@@ -296,12 +298,34 @@ class MixerSource {
         return std::nullopt;
     }
     void try_seek(Duration) { throw Error(RB_ERR_NOT_SUPPORTED_SEEK, "MixerSource::try_seek"); }   // mixer.rs:109-113
+    // Adapters on the MixerSource itself (rb_batch_set_master): [amplify] [limit] [amplify], over the whole mix.  A new handle
+    // on the same mixer, like rodio's adapters that take the source by value.
+    MixerSource amplify(float value) const {                                                                // amplify.rs:63-65
+        rb_effect e{};
+        e.kind = RB_FX_AMPLIFY, e.f32[0] = value;
+        return with(e);
+    }
+    MixerSource limit(const LimitSettings& ls = {}) const {                                                 // limit.rs:94-130
+        rb_effect e{};
+        e.kind = RB_FX_LIMIT, e.f32[0] = ls.threshold, e.f32[1] = ls.knee_width;
+        e.ns[0] = (uint64_t)ls.attack.count(), e.ns[1] = (uint64_t)ls.release.count();
+        return with(e);
+    }
 
   private:
+    MixerSource with(const rb_effect& e) const {
+        MixerSource m = *this;
+        m.master_.push_back(e);
+        return m;
+    }
+    static bool same(const std::vector<rb_effect>& a, const std::vector<rb_effect>& b) {
+        return a.size() == b.size() && (a.empty() || std::memcmp(a.data(), b.data(), a.size() * sizeof(rb_effect)) == 0);
+    }
     void render() {
         Shared& s = *s_;
-        if (!s.dirty) return;
+        if (!s.dirty && same(s.rendered_master, master_)) return;
         s.dirty = false;
+        s.rendered_master = master_;
         s.rendered.clear(), s.active.clear();
         if (s.sources.empty()) return;
         std::vector<const Source*> ptrs;
@@ -309,6 +333,7 @@ class MixerSource {
         detail::Flat flat(ptrs, s.starts);
         detail::Batch b(flat.descs, s.channels, s.rate, 0);
         flat.upload(b.h);
+        if (!master_.empty()) check(rb_batch_set_master(b.h, master_.data(), (uint32_t)master_.size()), "rb_batch_set_master");
         uint64_t n = 0, w = 0;
         check(rb_batch_mix_len(b.h, &n), "rb_batch_mix_len");
         s.rendered.resize(n);
@@ -322,6 +347,7 @@ class MixerSource {
         }
     }
     std::shared_ptr<Shared> s_;
+    std::vector<rb_effect> master_;
 };
 
 // mixer::mixer(channels, sample_rate) -> (Mixer, MixerSource) — src/mixer.rs:25-43
@@ -365,6 +391,10 @@ class LiveMixer {
     void set_amplify(size_t i, float factor) { check(rb_session_set_amplify(h_, i, factor), "rb_session_set_amplify"); }
     // Player::set_volume: the AMPLIFY in front of the mixer's conversion (src/player.rs:120-128, :180-186)
     void set_volume(size_t i, float factor) { check(rb_session_set_volume(h_, i, factor), "rb_session_set_volume"); }
+    // mixer_source.amplify(a).limit(s).amplify(b) on the output (rb_session_set_master), before the first next()
+    void set_master(const std::vector<rb_effect>& effects) {
+        check(rb_session_set_master(h_, effects.data(), (uint32_t)effects.size()), "rb_session_set_master");
+    }
     bool ended() const { return ended_ && at_ == block_.size(); }
     std::optional<Sample> next() {
         if (at_ == block_.size()) {

@@ -87,6 +87,8 @@ SYMBOLS = {
     "rb_batch_launches_per_render": (C.c_int32, [C.c_void_p, C.POINTER(C.c_uint32)]),
     "rb_batch_kernel_family": (C.c_int32, [C.c_void_p, C.POINTER(C.c_int)]),
     "rb_batch_mix_group": (C.c_int32, [C.c_void_p, C.POINTER(C.c_uint32)]),
+    "rb_batch_set_master": (C.c_int32, [C.c_void_p, C.POINTER(rb_effect), C.c_uint32]),
+    "rb_session_set_master": (C.c_int32, [C.c_void_p, C.POINTER(rb_effect), C.c_uint32]),
     "rb_wav_parse": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p]),
     "rb_wav_unpack24": (None, [C.c_void_p, C.c_uint64, C.c_void_p]),
     "rb_comm_unique_id": (C.c_int32, [C.c_void_p]),

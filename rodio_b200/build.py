@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "librodio_b200.so")
-SOURCES = ["rb_api.cu", "rb_kernels.cu", "rb_fused.cu", "rb_fx.cu", "rb_lanes.cu", "rb_lanes_batch.cu", "rb_p2p.cu"]
+SOURCES = ["rb_api.cu", "rb_kernels.cu", "rb_fused.cu", "rb_fx.cu", "rb_lanes.cu", "rb_lanes_batch.cu", "rb_p2p.cu", "rb_master.cu"]
 HEADERS = ["rb_internal.h", "rb_dsp.cuh", "rb_fused.h", "rb_fused_rows.h", "rb_lanes.h", "rb_lanes_core.h", "rb_duo_core.h", "rb_lanes_plan.h", "rb_session_plan.h", "rb_simt.h", "rb_p2p.h", os.path.join("..", "..", "include", "rodio_b200.h")]
 
 NVCC_FLAGS = [

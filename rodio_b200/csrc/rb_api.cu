@@ -20,6 +20,9 @@
 #include "rb_lanes_plan.h"
 #include "rb_session_plan.h"
 #include "rb_p2p.h"
+#if defined(RB_SIMT_EMULATE)
+#include "rb_master_host.h"   // the CPU build of the host code (tests/emu/): k_master's arithmetic in host form
+#endif
 
 // ------------------------------------------------------------------------------------------------
 // errors
@@ -128,6 +131,32 @@ static uint32_t f32_as_u32(float v) {  // Rust `as u32`
     return (uint32_t)v;
 }
 }  // namespace hostmath
+
+// RB_FX_LIMIT -> the limiter's coefficients at `rate` (limit.rs:94-130, :877)
+static rb_lim_params limit_params(const rb_effect& e, uint32_t rate) {
+    rb_lim_params l;
+    l.threshold = e.f32[0], l.knee = e.f32[1];
+    volatile float k8 = 8.0f * e.f32[1];
+    l.inv_knee_8 = 1.0f / k8;
+    l.attack = hostmath::duration_to_coefficient(e.ns[0], rate);
+    l.release = hostmath::duration_to_coefficient(e.ns[1], rate);
+    return l;
+}
+
+// Adapters on the MixerSource: [AMPLIFY] [LIMIT] [AMPLIFY], each optional, at least one; the limiter is built for the mixer's
+// rate (its channel count and rate never change: MixerSource::current_span_len() is None, mixer.rs:89-91).
+static rb_status parse_master(const rb_effect* fx, uint32_t n, uint32_t mixer_rate, rb_master_params* out) {
+    if (n && !fx) return fail(RB_ERR_INVALID_ARGUMENT, "effects is NULL");
+    rb_master_params p{};
+    p.pre = p.post = 1.0f;
+    uint32_t i = 0;
+    if (i < n && fx[i].kind == RB_FX_AMPLIFY) p.has_pre = 1, p.pre = fx[i++].f32[0];
+    if (i < n && fx[i].kind == RB_FX_LIMIT) p.has_lim = 1, p.lim = limit_params(fx[i++], mixer_rate);
+    if (i < n && fx[i].kind == RB_FX_AMPLIFY) p.has_post = 1, p.post = fx[i++].f32[0];
+    if (i != n) return fail(RB_ERR_UNSUPPORTED, "master chain: [AMPLIFY] [LIMIT] [AMPLIFY] on the MixerSource, nothing else");
+    *out = p;
+    return RB_OK;
+}
 
 // ---- WAV ingest: where the samples are and what they are (src/decoder/wav.rs:119-151 names the formats rodio reads) ----
 extern "C" rb_status rb_wav_parse(const void* image, uint64_t n, rb_wav_info* out) {
@@ -497,11 +526,7 @@ static rb_status plan_varying(PlanStream& ps, std::vector<SeqSeg> segs, size_t f
                 // coefficients (of the rate at construction) stay
                 rb_node_dev base{};
                 base.kind = RB_N_LIMIT, base.c_in = base.c_out = c0;
-                base.p.lim.threshold = e.f32[0], base.p.lim.knee = e.f32[1];
-                volatile float k8 = 8.0f * e.f32[1];
-                base.p.lim.inv_knee_8 = 1.0f / k8;
-                base.p.lim.attack = hostmath::duration_to_coefficient(e.ns[0], segs[0].r);
-                base.p.lim.release = hostmath::duration_to_coefficient(e.ns[1], segs[0].r);
+                base.p.lim = limit_params(e, segs[0].r);
                 nd.d = base;
                 nd.d.n_in = nd.d.n_out = n;
                 uint64_t from = 0;
@@ -729,11 +754,7 @@ static rb_status plan_stream(PlanStream& ps, uint16_t mixer_ch, uint32_t mixer_r
             }
             case RB_FX_LIMIT: {
                 nd.d.kind = RB_N_LIMIT;
-                nd.d.p.lim.threshold = e.f32[0], nd.d.p.lim.knee = e.f32[1];
-                volatile float k8 = 8.0f * e.f32[1];
-                nd.d.p.lim.inv_knee_8 = 1.0f / k8;   // limit.rs:877
-                nd.d.p.lim.attack = hostmath::duration_to_coefficient(e.ns[0], rate);
-                nd.d.p.lim.release = hostmath::duration_to_coefficient(e.ns[1], rate);
+                nd.d.p.lim = limit_params(e, rate);
                 break;
             }
             case RB_FX_SPATIAL:
@@ -917,6 +938,13 @@ struct rb_batch {
     uint32_t launches = 0;
     bool rendered = false;
     std::vector<uint8_t> uploaded;
+    // adapters on the MixerSource (rb_batch_set_master), run in place on d_out behind the mix
+    std::vector<rb_master_run> master_runs;   // the active runs of the mix, known from the closed-form lengths
+    uint64_t master_seq = 0;                  // samples in them
+    bool runs_aligned = true;                 // every run ends on a frame boundary
+    bool has_master = false;
+    rb_master_params master{};
+    rb_master_run* d_master_runs = nullptr;
 };
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -937,6 +965,7 @@ extern "C" rb_status rb_batch_destroy(rb_batch* b) {
     cudaFree(b->d_mix);
     cudaFree(b->d_mix_partial);
     cudaFree(b->d_out);
+    cudaFree(b->d_master_runs);
     delete b;
     return RB_OK;
 }
@@ -998,6 +1027,21 @@ extern "C" rb_status rb_batch_create(rb_context* ctx, uint16_t mixer_ch, uint32_
     }
     b->mix_len = mix_len;
     b->algo_bytes = algo + mix_len * 4;
+    {   // active runs: MixerSource::next() is Some where a source plays (mixer.rs:120-136); the gaps between are written as 0.0
+        std::vector<std::pair<uint64_t, uint64_t>> iv;
+        for (const PlanStream& ps : b->streams)
+            if (ps.out_len && !ps.consumed && ps.appended_to < 0) iv.push_back({ps.mix_start, ps.mix_start + ps.out_len});
+        std::sort(iv.begin(), iv.end());
+        uint64_t seq = 0;
+        for (size_t i = 0; i < iv.size();) {
+            uint64_t lo = iv[i].first, hi = iv[i].second;
+            for (i++; i < iv.size() && iv[i].first <= hi; i++) hi = std::max(hi, iv[i].second);
+            b->runs_aligned = b->runs_aligned && lo % mixer_ch == 0 && hi % mixer_ch == 0;
+            b->master_runs.push_back({seq + (hi - lo), lo - seq});
+            seq += hi - lo;
+        }
+        b->master_seq = seq;
+    }
     b->in_bytes = in_bytes;
 
     RB_CUDA(cudaMalloc(&b->d_in, std::max<size_t>(in_bytes, 256)));
@@ -1260,7 +1304,28 @@ extern "C" rb_status rb_batch_mix_len(rb_batch* b, uint64_t* n) {
 }
 extern "C" rb_status rb_batch_launches_per_render(rb_batch* b, uint32_t* n) {
     if (!b || !n) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
-    *n = b->launches;
+    *n = b->launches + (b->has_master && b->master_seq ? 1u : 0u);
+    return RB_OK;
+}
+extern "C" rb_status rb_batch_set_master(rb_batch* b, const rb_effect* effects, uint32_t n_effects) {
+    if (!b) return fail(RB_ERR_INVALID_ARGUMENT, "batch is NULL");
+    rb_master_params p{};
+    rb_status s = parse_master(effects, n_effects, b->mixer_rate, &p);
+    if (s != RB_OK) return s;
+    if (n_effects == 0) {
+        b->has_master = false;
+        return RB_OK;
+    }
+    // Limit::next keeps its channel position across a gap (it is not pulled there): a run that ends inside a frame would
+    // shift every later frame's channels, which the kernel's frame tiles do not follow
+    if (!b->runs_aligned)
+        return fail(RB_ERR_UNALIGNED_FRAMES, "master chain: an active run of the mix ends inside a frame (a chain with a trailing partial frame)");
+    if (!b->d_master_runs && !b->master_runs.empty()) {
+        RB_CUDA(cudaSetDevice(b->ctx->device));
+        RB_CUDA(cudaMalloc(&b->d_master_runs, b->master_runs.size() * sizeof(rb_master_run)));
+        RB_CUDA(cudaMemcpy(b->d_master_runs, b->master_runs.data(), b->master_runs.size() * sizeof(rb_master_run), cudaMemcpyHostToDevice));
+    }
+    b->master = p, b->has_master = true;
     return RB_OK;
 }
 extern "C" rb_status rb_batch_kernel_family(rb_batch* b, int* family) {
@@ -1311,6 +1376,9 @@ static rb_status render_device(rb_batch* b, bool skip_final_sum) {
         rb_status s = run_general(b, true);
         if (s != RB_OK) return s;
     }
+    if (b->has_master)
+        RB_CUDA(rb_launch_master(b->d_out, b->d_master_runs, (uint32_t)b->master_runs.size(), b->master_seq, b->mixer_ch, b->master, nullptr,
+                                 nullptr, b->ctx->stream));
     b->rendered = true;
     return RB_OK;
 }
@@ -1486,6 +1554,8 @@ static void comm_setup_p2p(rb_comm* c, NcclApi* api, uint64_t mix_len) {
 // each rb_batch_mix_device_ptr holds the sum over ALL ranks.  Asynchronous on the contexts' streams like a render.
 extern "C" rb_status rb_batch_render_mix_allreduce(rb_batch** batches, int n_local, rb_comm* c) {
     if (!batches || !c || n_local != (int)c->comms.size()) return fail(RB_ERR_INVALID_ARGUMENT, "one batch per local rank of the communicator");
+    for (int i = 0; i < n_local; i++)
+        if (batches[i] && batches[i]->has_master) return fail(RB_ERR_UNSUPPORTED, "a master chain runs on a single GPU's mix");
     NcclApi* api = nccl_api(nullptr);
     if (!api) return fail(RB_ERR_UNSUPPORTED, "NCCL is not loaded");
     for (int i = 0; i < n_local; i++) {
@@ -1689,6 +1759,14 @@ struct rb_session {
     lanes::Row* h_rows = nullptr;
     uint32_t* h_u32 = nullptr;
     float* h_out = nullptr;
+    // adapters on the MixerSource (rb_session_set_master).  The limiter state is double-buffered: a block reads
+    // d_master[master_k] and writes d_master[master_k ^ 1]; master_k flips once the block's synchronisation succeeded.
+    bool has_master = false;
+    rb_master_params master{};
+    float* d_master[2] = {nullptr, nullptr};   // integ[C], peak[C]
+    int master_k = 0;
+    rb_master_run* d_master_runs = nullptr;    // the block's active runs, [n_streams]
+    rb_master_run* h_master_runs = nullptr;
 };
 
 extern "C" rb_status rb_session_destroy(rb_session* s) {
@@ -1697,6 +1775,7 @@ extern "C" rb_status rb_session_destroy(rb_session* s) {
     cudaFree(s->d_fifo[0]), cudaFree(s->d_fifo[1]), cudaFree(s->d_state), cudaFree(s->d_zeros), cudaFree(s->d_partial);
     cudaFree(s->d_out), cudaFree(s->d_flags), cudaFree(s->d_rows), cudaFree(s->d_u32), cudaFree(s->d_off), cudaFree(s->d_stage);
     cudaFreeHost(s->h_rows), cudaFreeHost(s->h_u32), cudaFreeHost(s->h_out), cudaFreeHost(s->h_off);
+    cudaFree(s->d_master[0]), cudaFree(s->d_master[1]), cudaFree(s->d_master_runs), cudaFreeHost(s->h_master_runs);
     delete s;
     return RB_OK;
 }
@@ -1948,6 +2027,29 @@ extern "C" rb_status rb_session_set_volume(rb_session* s, size_t stream, float f
     return RB_OK;
 }
 
+extern "C" rb_status rb_session_set_master(rb_session* s, const rb_effect* effects, uint32_t n_effects) {
+    if (!s) return fail(RB_ERR_INVALID_ARGUMENT, "session is NULL");
+    if (s->T > 0) return fail(RB_ERR_STATE, "the master chain is set before the first rendered frame");
+    rb_master_params p{};
+    rb_status st = parse_master(effects, n_effects, s->mixer_rate, &p);
+    if (st != RB_OK) return st;
+    if (n_effects == 0) {
+        s->has_master = false;
+        return RB_OK;
+    }
+    RB_CUDA(cudaSetDevice(s->ctx->device));
+    const size_t ns = s->st.size();
+    if (!s->d_master[0]) {
+        for (int k = 0; k < 2; k++) RB_CUDA(cudaMalloc(&s->d_master[k], 2 * RB_MAX_CHANNELS * sizeof(float)));
+        RB_CUDA(cudaMalloc(&s->d_master_runs, ns * sizeof(rb_master_run)));
+        RB_CUDA(cudaMallocHost(&s->h_master_runs, ns * sizeof(rb_master_run)));
+    }
+    RB_CUDA(cudaMemsetAsync(s->d_master[s->master_k], 0, 2 * RB_MAX_CHANNELS * sizeof(float), s->ctx->stream));
+    RB_CUDA(cudaStreamSynchronize(s->ctx->stream));
+    s->master = p, s->has_master = true;
+    return RB_OK;
+}
+
 extern "C" rb_status rb_session_available(rb_session* s, uint64_t* frames, int* ended) {
     if (!s || !frames) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
     bool e = false;
@@ -2005,6 +2107,24 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
         g0 += a.n_groups;
     }
     RB_CUDA(rb_lanes_launch_sum(s->d_partial, n_groups_total, pstride, n * C, s->d_out, stq));
+    if (s->has_master) {
+        // the block's active runs: frames some source covers.  A frame no source covers (a source declared to join later, the
+        // others ended) is a gap: MixerSource::next() is None there, the chain is not pulled and the frame stays 0.0.
+        std::vector<std::pair<uint64_t, uint64_t>> iv;
+        for (size_t r = 0; r < ns; r++)
+            if (parts[r].out_len) iv.push_back({parts[r].mix_start, parts[r].mix_start + parts[r].out_len});
+        std::sort(iv.begin(), iv.end());
+        uint32_t n_runs = 0;
+        uint64_t seq = 0;
+        for (size_t i = 0; i < iv.size();) {
+            uint64_t lo = iv[i].first, hi = iv[i].second;
+            for (i++; i < iv.size() && iv[i].first <= hi; i++) hi = std::max(hi, iv[i].second);
+            s->h_master_runs[n_runs++] = {(seq + hi - lo) * C, (lo - seq) * C};
+            seq += hi - lo;
+        }
+        if (n_runs) RB_CUDA(cudaMemcpyAsync(s->d_master_runs, s->h_master_runs, n_runs * sizeof(rb_master_run), cudaMemcpyHostToDevice, stq));
+        RB_CUDA(rb_launch_master(s->d_out, s->d_master_runs, n_runs, seq * C, C, s->master, s->d_master[s->master_k], s->d_master[s->master_k ^ 1], stq));
+    }
     // the host already knows what every stream consumed: compact the FIFOs into the other arena behind the kernel.
     // The bookkeeping is advanced here and committed by the synchronisation below: when a CUDA call in between fails, the
     // snapshot comes back, so that FIFO positions, volumes and T never run ahead of what the device has done.
@@ -2036,6 +2156,7 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
     RB_CUDA_TX(cudaMemcpyAsync(s->h_out, s->d_out, n * C * sizeof(float), cudaMemcpyDeviceToHost, stq));
     RB_CUDA_TX(cudaStreamSynchronize(stq));
 #undef RB_CUDA_TX
+    if (s->has_master) s->master_k ^= 1;
     memcpy(out_host, s->h_out, n * C * sizeof(float));
     s->T += n;
     *written = n;
@@ -2063,6 +2184,12 @@ struct SessionBlobStream {   // in class order (the same descriptors give the sa
     uint32_t held;                       // still waiting for rb_session_start / its predecessor (RB_SESSION_HELD)
     int32_t follows;                     // class-order index of the source it is queued behind (rb_session_follow), -1: none
 };
+// Behind the FIFO contents when the session has a master chain (header pad_ = 1); without one the blob ends with them.
+struct SessionBlobMaster {
+    rb_master_params params;             // a blob only restores a session with the same chain
+    uint32_t channels;
+    float integ[RB_MAX_CHANNELS], peak[RB_MAX_CHANNELS];
+};
 constexpr uint32_t SESSION_MAGIC = 0x52425353u;   // "RBSS"
 }  // namespace
 
@@ -2072,6 +2199,7 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
     uint64_t need = sizeof(SessionBlobHeader) + ns * sizeof(SessionBlobStream);
     const uint32_t C = s->channels;
     for (size_t r = 0; r < ns; r++) need += s->st[r].fill() * s->src_ch[r] * sizeof(float);
+    if (s->has_master) need += sizeof(SessionBlobMaster);
     *size = need;
     if (!buf) return RB_OK;
     if (cap < need) return fail(RB_ERR_BUFFER_TOO_SMALL, "state buffer too small");
@@ -2080,8 +2208,11 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
     std::vector<uint32_t> flags(ns);
     RB_CUDA(cudaMemcpyAsync(state.data(), s->d_state, 4 * C * ns * sizeof(float), cudaMemcpyDeviceToHost, s->ctx->stream));
     RB_CUDA(cudaMemcpyAsync(flags.data(), s->d_flags, ns * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->ctx->stream));
+    float mstate[2 * RB_MAX_CHANNELS] = {0};
+    if (s->has_master)
+        RB_CUDA(cudaMemcpyAsync(mstate, s->d_master[s->master_k], 2 * C * sizeof(float), cudaMemcpyDeviceToHost, s->ctx->stream));
     uint8_t* p = (uint8_t*)buf;
-    SessionBlobHeader h{SESSION_MAGIC, 5u, (uint32_t)ns, s->has_biquad ? 1u : 0u, C, 0u, s->T};
+    SessionBlobHeader h{SESSION_MAGIC, 5u, (uint32_t)ns, s->has_biquad ? 1u : 0u, C, s->has_master ? 1u : 0u, s->T};
     memcpy(p, &h, sizeof(h)), p += sizeof(h);
     uint8_t* recs = p;
     p += ns * sizeof(SessionBlobStream);
@@ -2097,6 +2228,12 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
                             st.front ? s->mid[r] : s->pre[r], s->post[r], st.held ? 1u : 0u, (int32_t)st.follows};
         for (uint32_t k = 0; k < 4 * C; k++) b.state[k] = state[4 * C * r + k];
         memcpy(recs + r * sizeof(b), &b, sizeof(b));
+    }
+    if (s->has_master) {
+        SessionBlobMaster m{};
+        m.params = s->master, m.channels = C;
+        for (uint32_t c = 0; c < C; c++) m.integ[c] = mstate[c], m.peak[c] = mstate[C + c];
+        memcpy(p, &m, sizeof(m));
     }
     return RB_OK;
 }
@@ -2127,6 +2264,15 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
             return fail(RB_ERR_INVALID_ARGUMENT, "state blob: more outputs rendered than the pushed input holds");
         need += (uint64_t)b.fill * s->src_ch[r] * sizeof(float);
     }
+    if (h.pad_ != (s->has_master ? 1u : 0u)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session with another master chain");
+    SessionBlobMaster m{};
+    if (s->has_master) {
+        if (size < need + sizeof(m)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
+        memcpy(&m, (const uint8_t*)buf + need, sizeof(m));
+        need += sizeof(m);
+        if (m.channels != C || memcmp(&m.params, &s->master, sizeof(m.params)) != 0)
+            return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session with another master chain");
+    }
     if (size < need) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
     RB_CUDA(cudaSetDevice(s->ctx->device));
     std::vector<float> state(4 * C * ns);
@@ -2146,6 +2292,11 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
     }
     RB_CUDA(cudaMemcpyAsync(s->d_state, state.data(), 4 * C * ns * sizeof(float), cudaMemcpyHostToDevice, s->ctx->stream));
     RB_CUDA(cudaMemcpyAsync(s->d_flags, flags.data(), ns * sizeof(uint32_t), cudaMemcpyHostToDevice, s->ctx->stream));
+    float mstate[2 * RB_MAX_CHANNELS];
+    if (s->has_master) {
+        for (uint32_t c = 0; c < C; c++) mstate[c] = m.integ[c], mstate[C + c] = m.peak[c];
+        RB_CUDA(cudaMemcpyAsync(s->d_master[s->master_k], mstate, 2 * C * sizeof(float), cudaMemcpyHostToDevice, s->ctx->stream));
+    }
     RB_CUDA(cudaStreamSynchronize(s->ctx->stream));
     s->T = h.T;
     return RB_OK;

@@ -53,6 +53,9 @@ struct rb_uniform_params {
     rb_uniform_seg tail;          // the last, shorter chunk (or the whole input)
 };
 
+// Limiter coefficients (src/source/limit.rs:94-130, :854-988); attack / release for the rate the limiter was built at.
+struct rb_lim_params { float threshold, knee, inv_knee_8, attack, release; };
+
 // One adapter applied to one stream, as the device sees it.  POD, 16-byte aligned.
 struct alignas(16) rb_node_dev {
     const void* src;       // f32 except for RB_N_CONVERT
@@ -74,7 +77,7 @@ struct alignas(16) rb_node_dev {
         } blt;
         struct { uint64_t delay; float amplitude; } echo;
         struct { float target, max_gain, floor, attack, release; } agc;
-        struct { float threshold, knee, inv_knee_8, attack, release; } lim;
+        rb_lim_params lim;
         struct { float vol[RB_MAX_CHANNELS]; } cv;
         struct { float gain, threshold; } dist;
         struct { uint64_t total_ns, dt_ns; float start, end; uint32_t clamp_end; } ramp;
@@ -102,3 +105,20 @@ cudaError_t rb_launch_mix(const rb_mix_src* d_srcs, uint32_t n_srcs, float* d_ou
                           float* d_partial = nullptr, uint32_t n_groups = 1);
 cudaError_t rb_launch_convert(const void* d_in, uint32_t in_fmt, void* d_out, uint32_t out_fmt, uint64_t n,
                               cudaStream_t st);
+
+// ---- adapters on the MixerSource itself: Amplify(Limit(Amplify(mix))), each stage optional (rb_master.cu) ----
+struct rb_master_params {
+    float pre, post;                     // 1.0 where the AMPLIFY is absent
+    uint32_t has_pre, has_lim, has_post;
+    rb_lim_params lim;                   // built for the mixer's rate
+};
+// The active runs of the mix (where MixerSource::next() returns Some) are one sequence for the chain; a gap is not pulled.
+// Run r covers sequence samples [runs[r-1].seq_end, runs[r].seq_end) at mix samples seq + runs[r].delta.
+struct rb_master_run {
+    uint64_t seq_end;
+    uint64_t delta;
+};
+// In place on `mix`.  n_seq = total samples of the runs (whole frames of `channels`).  state_in: integ[channels] then
+// peak[channels] (nullptr: zero, a new limiter); state_out (may be nullptr) receives the state after the last frame.
+cudaError_t rb_launch_master(float* mix, const rb_master_run* d_runs, uint32_t n_runs, uint64_t n_seq, uint32_t channels,
+                             const rb_master_params& p, const float* state_in, float* state_out, cudaStream_t st);

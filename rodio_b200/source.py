@@ -137,6 +137,31 @@ class LimitSettings:
 # ---------------------------------------------------------------------------------------------
 # trait Source (src/source/mod.rs:179-759): PCM + recorded adapter chain
 # ---------------------------------------------------------------------------------------------
+def amplify_effect(value: float) -> Effect:
+    """The record of Source::amplify / MixerSource::amplify (src/source/amplify.rs:63-65)."""
+    return Effect.make(capi.RB_FX_AMPLIFY, f32=[value])
+
+
+def limit_effect(settings: Optional[LimitSettings] = None) -> Effect:
+    """The record of Source::limit / MixerSource::limit (src/source/limit.rs:94-130)."""
+    s = settings or LimitSettings()
+    return Effect.make(capi.RB_FX_LIMIT, f32=[s.threshold, s.knee_width], ns=[s.attack, s.release])
+
+
+def effect_records(effects: Sequence[Effect]):
+    """The rb_effect array of a master chain (adapters on the MixerSource: rb_batch_set_master / rb_session_set_master)."""
+    fx = (capi.rb_effect * max(1, len(effects)))()
+    for j, e in enumerate(effects):
+        fx[j].kind = e.kind
+        for k in range(3):
+            fx[j].u32[k] = e.u32[k]
+        for k in range(12):
+            fx[j].f32[k] = e.f32[k]
+        for k in range(2):
+            fx[j].ns[k] = e.ns[k]
+    return fx
+
+
 class Source:
     def __init__(self, pcm: np.ndarray, channels: int, sample_rate: int, span_len: int,
                  effects: Optional[List[Effect]] = None, cur_channels: Optional[int] = None,
@@ -172,7 +197,7 @@ class Source:
     # -- adapters ---------------------------------------------------------------------------
     def amplify(self, value: float) -> "Source":
         """Source::amplify — src/source/mod.rs:307-314."""
-        return self._with(Effect.make(capi.RB_FX_AMPLIFY, f32=[value]))
+        return self._with(amplify_effect(value))
 
     def amplify_decibel(self, value: float) -> "Source":
         """Source::amplify_decibel — src/source/mod.rs:316-323 (math::db_to_linear)."""
@@ -258,8 +283,7 @@ class Source:
 
     def limit(self, settings: Optional[LimitSettings] = None) -> "Source":
         """Source::limit — src/source/limit.rs:94-130."""
-        s = settings or LimitSettings()
-        return self._with(Effect.make(capi.RB_FX_LIMIT, f32=[s.threshold, s.knee_width], ns=[s.attack, s.release]))
+        return self._with(limit_effect(settings))
 
     # -- draining ----------------------------------------------------------------------------
     def collect(self, ctx: Optional["Context"] = None) -> np.ndarray:
@@ -545,13 +569,20 @@ class Batch:
     """mixer(channels, rate) + Mixer::add for every source, as one rb_batch."""
 
     def __init__(self, sources: Sequence[Source], mixer_channels: int, mixer_rate: int, flags: int = 0,
-                 mix_starts: Optional[Sequence[int]] = None, ctx: Optional[Context] = None):
+                 mix_starts: Optional[Sequence[int]] = None, ctx: Optional[Context] = None, master: Sequence[Effect] = ()):
+        """master: adapters on the MixerSource itself, [amplify] [limit] [amplify] (rb_batch_set_master)."""
         self.ctx = ctx or default_context()
         self._descs, self._keep = pack_descs(list(sources), mix_starts)
         self.sources = self._keep[0]          # the sources handed in, then the second inputs of their mix() adapters
         self._h = C.c_void_p()
         check(lib().rb_batch_create(self.ctx._h, mixer_channels, mixer_rate, self._descs, len(self.sources), flags,
                                     C.byref(self._h)), "rb_batch_create")
+        if master:
+            try:
+                check(lib().rb_batch_set_master(self._h, effect_records(master), len(master)), "rb_batch_set_master")
+            except Exception:
+                self.close()
+                raise
 
     def close(self):
         if self._h:
@@ -666,7 +697,9 @@ class Session:
     (UniformSourceIterator(src, 1, rate)[.low_pass / .high_pass][.amplify]); their pcm is ignored."""
 
     def __init__(self, sources: Sequence[Source], mixer_rate: int, fifo_frames: int = 8192, max_block_frames: int = 4096,
-                 mix_starts: Optional[Sequence[int]] = None, ctx: Optional[Context] = None, mixer_channels: Optional[int] = None):
+                 mix_starts: Optional[Sequence[int]] = None, ctx: Optional[Context] = None, mixer_channels: Optional[int] = None,
+                 master: Sequence[Effect] = ()):
+        """master: adapters on the mixer's output, [amplify] [limit] [amplify] (rb_session_set_master)."""
         self.ctx = ctx or default_context()
         self.sources = list(sources)
         self.max_block_frames = max_block_frames
@@ -677,6 +710,16 @@ class Session:
         self._h = C.c_void_p()
         check(lib().rb_session_create(self.ctx._h, self.channels, mixer_rate, self._descs, len(self.sources), fifo_frames,
                                       max_block_frames, C.byref(self._h)), "rb_session_create")
+        if master:
+            try:
+                self.set_master(master)
+            except Exception:
+                self.close()
+                raise
+
+    def set_master(self, effects: Sequence[Effect]):
+        """mixer_source.amplify(a).limit(s).amplify(b) on the output; before the first rendered frame."""
+        check(lib().rb_session_set_master(self._h, effect_records(effects), len(effects)), "rb_session_set_master")
 
     def close(self):
         if self._h:
@@ -759,6 +802,7 @@ class _MixerShared:
         self.pos = 0              # samples already handed out by MixerSource
         self.rendered: Optional[np.ndarray] = None
         self.active: Optional[np.ndarray] = None
+        self.rendered_master: Tuple[Effect, ...] = ()   # the MixerSource adapters `rendered` went through
 
 
 class Mixer:
@@ -777,8 +821,19 @@ class Mixer:
 class MixerSource:
     """The output (`mixer::MixerSource`, src/mixer.rs:70-136): an iterator of f32 that implements Source."""
 
-    def __init__(self, shared: _MixerShared):
+    def __init__(self, shared: _MixerShared, master: Tuple[Effect, ...] = ()):
         self._s = shared
+        self._master = tuple(master)
+
+    # -- adapters on the MixerSource itself: [amplify] [limit] [amplify] (rb_batch_set_master), over the whole mix ----------
+    def amplify(self, value: float) -> "MixerSource":
+        """Source::amplify on the mixer's output (src/source/amplify.rs:63-65).  A new handle on the same mixer: rodio's
+        adapters take the source by value."""
+        return MixerSource(self._s, self._master + (amplify_effect(value),))
+
+    def limit(self, settings: Optional[LimitSettings] = None) -> "MixerSource":
+        """Source::limit on the mixer's output (src/source/limit.rs:94-130), built for the mixer's channels and rate."""
+        return MixerSource(self._s, self._master + (limit_effect(settings),))
 
     def channels(self) -> int:
         return self._s.channels
@@ -795,13 +850,14 @@ class MixerSource:
 
     def _render(self):
         s = self._s
-        if s.rendered is not None:
+        if s.rendered is not None and s.rendered_master == self._master:
             return
+        s.rendered_master = self._master
         if not s.sources:
             s.rendered = np.zeros(0, dtype=np.float32)
             s.active = np.zeros(0, dtype=bool)
             return
-        with Batch(s.sources, s.channels, s.rate, flags=s.flags, mix_starts=s.starts, ctx=s.ctx) as b:
+        with Batch(s.sources, s.channels, s.rate, flags=s.flags, mix_starts=s.starts, ctx=s.ctx, master=self._master) as b:
             b.upload_all()
             s.rendered = b.render_mix()
             act = np.zeros(s.rendered.size + 1, dtype=np.int64)
