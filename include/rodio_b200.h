@@ -323,9 +323,17 @@ rb_status rb_batch_read_stream(rb_batch* b, size_t stream, float* out_host, uint
  * PCM is pushed per source as it arrives, the mixer output is pulled in blocks; the resampler position, the input
  * frames still needed and the filter state carry over from block to block, so ANY split into pushes and renders gives
  * the bytes of a whole-stream rb_batch render with RB_FUSED_LANES (tests/test_lanes_emulator.py::test_session_*).
- * Shape served (RB_ERR_UNSUPPORTED otherwise): a mono or stereo mixer = mixer(channels, rate) of src/mixer.rs:25-43; f32
- * sources with the mixer's channel count or mono sources in a stereo mixer (repeated on both channels like
- * ChannelCountConverter, src/conversions/channels.rs:57-85), each at its own sample rate (44.1 kHz, 22.05 kHz and 48 kHz sources in one 48 kHz mixer: one kernel launch
+ * Shape served (RB_ERR_UNSUPPORTED otherwise): a mixer of 1 to 12 channels = mixer(channels, rate) of src/mixer.rs:25-43 (the
+ * device's channel count, src/stream.rs); f32 sources of 1 to 12 channels each (a mono mixer: mono sources only), brought to
+ * the mixer's count like ChannelCountConverter (src/conversions/channels.rs:57-85): output channel j is input channel j if j < the source's count,
+ * channel 0 again if j == 1 and the source is mono, else 0.0 -- a 5.1 source in a stereo mixer keeps its first two channels.
+ * A source whose conversion pads channels with 0.0 is refused when the filter behind the conversion has a non-finite
+ * coefficient or the gain behind it is not finite (rodio puts NaN on those channels; the session adds nothing there), and
+ * rb_session_set_amplify refuses a non-finite factor for it.  Mix order: a source is served as slot rows of at most two
+ * mixer channels each (channels 2s, 2s + 1; a mono source in a wider mixer: one row on channels 0 and 1); the rows of all
+ * sources, in the caller's order, form classes by rate pair, chain variant and slot; per class groups of 32 rows are summed
+ * with the lane kernel's tree, and mixer channel j is +0.0 plus every group whose slot covers j, in class order.  Each source
+ * is at its own sample rate (44.1 kHz, 22.05 kHz and 48 kHz sources in one 48 kHz mixer: one kernel launch
  * per rate pair; sources ABOVE the mixer's rate have fast tiles of their own up to a factor of two, the kernel's general per-sample path beyond), effects = [SPEED | AMPLIFY | one LOW_PASS / HIGH_PASS]* UNIFORM(mixer channels, mixer rate)
  * [LOW_PASS | HIGH_PASS] [AMPLIFY] -- the chain of BASELINE cfg3 behind the conversion, and in front of it what a rodio user
  * hands to Mixer::add or appends to a Player (src/player.rs:120-128): any SPEED (it only changes the rate pair), one filter
@@ -385,7 +393,9 @@ rb_status rb_session_available(rb_session* s, uint64_t* frames, int* ended);
 rb_status rb_session_render(rb_session* s, float* out_host, uint64_t max_frames, uint64_t* written, int* ended);
 /* Block-to-block state as an opaque blob -- resampler positions, pending input frames, filter state (the
  * rb_batch_get_state / rb_batch_set_state of SURVEY.md 8b): a session of the same shape restored from it, on any
- * context, continues bit-identically.  buf == NULL: only *size is returned. */
+ * context, continues bit-identically.  buf == NULL: only *size is returned.  One record per slot row; a session whose every
+ * source is one row carrying all of its channels (mono and stereo mixers, mono sources in any mixer) writes version 5, any
+ * other layout version 6 with a layout record per row.  A blob of another shape, layout or master chain: RB_ERR_INVALID_ARGUMENT. */
 rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap, uint64_t* size);
 rb_status rb_session_set_state(rb_session* s, const void* buf, uint64_t size);
 

@@ -22,6 +22,7 @@
 #include "rb_p2p.h"
 #if defined(RB_SIMT_EMULATE)
 #include "rb_master_host.h"   // the CPU build of the host code (tests/emu/): k_master's arithmetic in host form
+#include "rb_session_host.h"  // ... and the sessions' FIFO scatter and slot sum
 #endif
 
 // ------------------------------------------------------------------------------------------------
@@ -1725,39 +1726,59 @@ extern "C" rb_status rb_convert_samples(rb_context* ctx, const void* in, rb_samp
 // ------------------------------------------------------------------------------------------------
 // Bookkeeping: rb_session_plan.h (plain host code, also run by the CPU emulator of tests/emu/);
 // kernel: k_fused_lanes over per-block rows (rb_lanes_core.h: o0 / i0 / state / ROW_CONTINUES).
+// Slot rows: the lane kernel carries at most two channels per lane (CI == CO, or CI = 1 and CO = 2), so a source is served by
+// one row per pair of the mixer channels it feeds (rb_lanes.h, rb_fifo_job).  Output channel j of ChannelCountConverter
+// (src/conversions/channels.rs:57-85) is input channel j if j < CI, channel 0 again if j == 1 and CI == 1, else 0.0: the rows
+// cover every channel of the first kind and of the second; a channel of the third kind gets no row, because +-0 added to a
+// sum that starts from +0.0 changes nothing -- as long as the filter and the gain behind the conversion are finite
+// (rb_session_create refuses the other sources).
 struct rb_session {
     rb_context* ctx = nullptr;
     uint32_t mixer_rate = 0;
-    uint32_t channels = 1;        // of the mixer (1 or 2); a source has the same count, or is mono in a stereo mixer
-    std::vector<uint8_t> src_ch;  // per source (class order): its own channel count
+    uint32_t channels = 1;        // of the mixer (1 .. RB_MAX_CHANNELS)
+    std::vector<uint8_t> src_ch;  // per source (source order): its own channel count
+    std::vector<uint8_t> pads;    // per source: its conversion pads channels with 0.0
     bool has_biquad = false, has_post = false;
     // Sources may have different rates (each at or below the mixer's): one kernel launch per reduced rate pair.  All
-    // per-source arrays below are in CLASS ORDER (stable partition by rate pair); pos[] maps the caller's index to it.
-    struct Class {
-        uint32_t first = 0, count = 0, ch_in = 1;
-        bool has_biquad = false, ff2 = false, has_pre = false, front = false;
-    };
-    std::vector<Class> classes;
+    // per-source arrays below are in SOURCE ORDER (stable partition by rate pair, channels and chain variant); pos[] maps the
+    // caller's index to it.
     std::vector<uint32_t> pos;
     std::vector<session::Stream> st;
     std::vector<float> coef;      // 5 per stream
     std::vector<float> ffk, post, pre, mid;
     std::vector<float> vol_a, vol_b;   // the factor the two frames in front of Stream::fpos were pulled with (rb_session_set_volume)
+    // Rows are in CLASS ORDER: the rows of the sources in the caller's order, each source's slots in channel order, stably
+    // partitioned by (rate pair, chain variant, slot).  One launch per class; k_sum_slots adds the partial rows in that order.
+    // FIFOs, filter states and input flags are per row; positions, gains and the queue are per source.
+    struct Slot {
+        uint32_t src;             // source order
+        uint8_t ch0, w, ci;       // mixer channels [ch0, ch0 + w), fed by source channels [ch0, ch0 + ci) (ci = 1, w = 2: mono repeated)
+    };
+    struct Class {
+        uint32_t first = 0, count = 0, ch_in = 1, ch_out = 1;
+        bool has_biquad = false, ff2 = false, has_pre = false, front = false;
+    };
+    std::vector<Class> classes;
+    std::vector<Slot> rows;
+    std::vector<std::vector<uint32_t>> rows_of;   // per source: its rows, in slot order
+    bool plain = true;            // every source is one row that carries all of its channels: the version-5 state blob
+    uint32_t n_groups = 0;        // partial rows: one per warp, every class rounds up on its own
     uint64_t T = 0;               // mixer frames rendered so far
-    uint32_t fifo_cap = 0, max_block = 0;
-    uint64_t stride = 0;          // floats per stream in a FIFO arena
+    uint32_t fifo_cap = 0, max_block = 0, max_src_ch = 1;
+    uint64_t stride = 0;          // floats per row in a FIFO arena
     float* d_fifo[2] = {nullptr, nullptr};
     int cur = 0;
-    float *d_state = nullptr, *d_zeros = nullptr, *d_partial = nullptr, *d_out = nullptr;
-    uint32_t* d_flags = nullptr;  // sticky: a pushed frame was outside the exact-reciprocal class
+    float *d_state = nullptr, *d_zeros = nullptr, *d_partial = nullptr, *d_out = nullptr;   // d_state: 8 floats per row
+    uint32_t* d_flags = nullptr;  // per row, sticky: a pushed frame was outside the exact-reciprocal class
     lanes::Row* d_rows = nullptr;
-    uint32_t* d_u32 = nullptr;    // [2][n]: drop, keep (render) / count, fill (packed push)
-    uint64_t* d_off = nullptr;    // [n]: packed push offsets
-    float* d_stage = nullptr;     // packed push staging, [n * fifo_cap]
-    uint64_t* h_off = nullptr;
+    uint32_t* d_u32 = nullptr;    // [2][rows]: drop, keep (render)
+    uint32_t* d_slot = nullptr;   // per partial row: ch0 | w << 16 (k_sum_slots)
+    rb_fifo_job* d_jobs = nullptr;   // [rows]: the scatter of one push
+    float* d_stage = nullptr;     // push staging, [n * fifo_cap * max_src_ch], allocated by the first push
     // pinned host mirrors, reused by every call (each call ends with a stream synchronisation)
     lanes::Row* h_rows = nullptr;
     uint32_t* h_u32 = nullptr;
+    rb_fifo_job* h_jobs = nullptr;
     float* h_out = nullptr;
     // adapters on the MixerSource (rb_session_set_master).  The limiter state is double-buffered: a block reads
     // d_master[master_k] and writes d_master[master_k ^ 1]; master_k flips once the block's synchronisation succeeded.
@@ -1767,14 +1788,17 @@ struct rb_session {
     int master_k = 0;
     rb_master_run* d_master_runs = nullptr;    // the block's active runs, [n_streams]
     rb_master_run* h_master_runs = nullptr;
+#if defined(RB_SIMT_EMULATE)
+    std::vector<uint64_t> emu_fast_tiles;      // CPU build: fast tiles the emulator ran per class (rb_session_emu_fast_tiles)
+#endif
 };
 
 extern "C" rb_status rb_session_destroy(rb_session* s) {
     if (!s) return RB_OK;
     if (s->ctx) cudaSetDevice(s->ctx->device);
     cudaFree(s->d_fifo[0]), cudaFree(s->d_fifo[1]), cudaFree(s->d_state), cudaFree(s->d_zeros), cudaFree(s->d_partial);
-    cudaFree(s->d_out), cudaFree(s->d_flags), cudaFree(s->d_rows), cudaFree(s->d_u32), cudaFree(s->d_off), cudaFree(s->d_stage);
-    cudaFreeHost(s->h_rows), cudaFreeHost(s->h_u32), cudaFreeHost(s->h_out), cudaFreeHost(s->h_off);
+    cudaFree(s->d_out), cudaFree(s->d_flags), cudaFree(s->d_rows), cudaFree(s->d_u32), cudaFree(s->d_slot), cudaFree(s->d_jobs), cudaFree(s->d_stage);
+    cudaFreeHost(s->h_rows), cudaFreeHost(s->h_u32), cudaFreeHost(s->h_jobs), cudaFreeHost(s->h_out);
     cudaFree(s->d_master[0]), cudaFree(s->d_master[1]), cudaFree(s->d_master_runs), cudaFreeHost(s->h_master_runs);
     delete s;
     return RB_OK;
@@ -1785,7 +1809,7 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
     if (!ctx || !out || !descs) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
     if (mixer_rate == 0 || mixer_channels == 0 || n_streams == 0 || n_streams > 0x7FFFFFFFull)
         return fail(RB_ERR_INVALID_ARGUMENT, "zero mixer rate / channels or no streams");
-    if (mixer_channels > 2) return fail(RB_ERR_UNSUPPORTED, "sessions serve mono and stereo mixers");
+    if (mixer_channels > RB_MAX_CHANNELS) return fail(RB_ERR_UNSUPPORTED, "mixer: more than 12 channels");
     if (fifo_frames < 64 || max_block_frames == 0) return fail(RB_ERR_INVALID_ARGUMENT, "fifo_frames < 64 or max_block_frames == 0");
     if ((uint64_t)fifo_frames * RB_MAX_CHANNELS >= (1ull << 32))   // per-stream float counts travel as 32-bit words
         return fail(RB_ERR_OUT_OF_MEMORY, "fifo_frames too large (fifo_frames * channels must stay below 2^32)");
@@ -1802,8 +1826,8 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
         const std::string where = "stream " + std::to_string(i) + ": ";
         if (d.sample_rate == 0 || d.channels == 0) return fail(RB_ERR_INVALID_ARGUMENT, where + "zero sample rate or channels");
         if (d.format != RB_FMT_F32) return fail(RB_ERR_UNSUPPORTED, where + "sessions take f32 sources");
-        if (!(d.channels == mixer_channels || (d.channels == 1 && mixer_channels == 2)))
-            return fail(RB_ERR_UNSUPPORTED, where + "a source has the mixer's channel count, or is mono in a stereo mixer");
+        if (d.channels > RB_MAX_CHANNELS) return fail(RB_ERR_UNSUPPORTED, where + "more than 12 channels");
+        if (mixer_channels == 1 && d.channels != 1) return fail(RB_ERR_UNSUPPORTED, where + "a mono mixer takes mono sources");
         chs[i] = d.channels;
         if (d.n_effects && !d.effects) return fail(RB_ERR_INVALID_ARGUMENT, where + "effects is NULL");
         // Source::speed in front of the conversion only changes the rate the source reports (src/source/speed.rs:130-133);
@@ -1836,20 +1860,13 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
         if (from[i] > (1u << 20) || to[i] > (1u << 20))
             return fail(RB_ERR_RATIO_OVERFLOW, where + "reduced rate pair beyond 2^20");
     }
-    const auto classes = lanes::classes_by_ratio(from.data(), to.data(), key.data(), (uint32_t)n);
     s->pos.assign(n, 0);
-    std::vector<uint32_t> order;   // class order -> caller's index
-    for (const auto& cls : classes) {
-        rb_session::Class c;
-        c.first = (uint32_t)order.size(), c.count = (uint32_t)cls.size(), c.ch_in = chs[cls[0]];
-        c.front = (key[cls[0]] & 0x400u) != 0;
-        c.has_biquad = (key[cls[0]] & 0x100u) != 0 || c.front, c.has_pre = (key[cls[0]] & 0x200u) != 0;
+    std::vector<uint32_t> order;   // source order -> caller's index
+    for (const auto& cls : lanes::classes_by_ratio(from.data(), to.data(), key.data(), (uint32_t)n))
         for (uint32_t i : cls) s->pos[i] = (uint32_t)order.size(), order.push_back(i);
-        s->classes.push_back(c);
-    }
-    // pass 2: chains, in class order
+    // pass 2: chains, in source order
     s->st.resize(n), s->coef.assign(5 * n, 0.0f), s->ffk.assign(n, 0.0f), s->post.assign(n, 1.0f), s->pre.assign(n, 1.0f), s->mid.assign(n, 1.0f), s->src_ch.assign(n, 1);
-    s->vol_a.assign(n, 1.0f), s->vol_b.assign(n, 1.0f);
+    s->vol_a.assign(n, 1.0f), s->vol_b.assign(n, 1.0f), s->pads.assign(n, 0);
     bool any_biquad = false;
     std::vector<uint8_t> row_ff2(n, 1);
     for (size_t r = 0; r < n; r++) {
@@ -1869,6 +1886,7 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
             row_ff2[r] = 0, biq = true;
             s->st[r].front = true;
         }
+        bool behind = false;   // a filter behind the conversion: it also filters the channels the conversion pads
         if (k < d.n_effects && (d.effects[k].kind == RB_FX_LOW_PASS || d.effects[k].kind == RB_FX_HIGH_PASS)) {
             const rb_effect& e = d.effects[k];
             if (e.u32[0] == 0 || !(e.f32[0] > 0.0f)) return fail(RB_ERR_INVALID_ARGUMENT, where + "filter frequency and q must be positive");
@@ -1876,52 +1894,114 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
             float* co = &s->coef[5 * r];
             co[0] = c.b0, co[1] = c.b1, co[2] = c.b2, co[3] = c.a1, co[4] = c.a2;
             if (!lanes::ff2_coeffs(c.b0, c.b1, c.b2, &s->ffk[r])) row_ff2[r] = 0;
-            biq = true, k++;
+            biq = behind = true, k++;
         }
         any_biquad |= biq;
         if (k < d.n_effects && d.effects[k].kind == RB_FX_AMPLIFY) s->post[r] = d.effects[k].f32[0], s->has_post = true, k++;
         if (k != d.n_effects) return fail(RB_ERR_UNSUPPORTED, where + "chain shape: [SPEED | AMPLIFY | one filter] UNIFORM [LOW_PASS | HIGH_PASS] [AMPLIFY]");
+        // Channels the conversion pads get no row: their 0.0 must stay a zero behind the filter and the gain
+        s->pads[r] = mixer_channels > (d.channels == 1 ? 2u : d.channels);
+        if (s->pads[r]) {
+            const float* co = &s->coef[5 * r];
+            bool finite = std::isfinite(s->post[r]);
+            for (int j = 0; j < 5 && behind; j++) finite = finite && std::isfinite(co[j]);
+            if (!finite)
+                return fail(RB_ERR_UNSUPPORTED, where + "the conversion pads channels with 0.0 and the filter or gain behind it is not finite (rodio gives NaN there)");
+        }
         s->st[r].mix_start = d.mix_start, s->st[r].from = from[i], s->st[r].to = to[i];
         if (d.mix_start == RB_SESSION_HELD) s->st[r].held = true, s->st[r].mix_start = 0;   // Mixer::add comes later (rb_session_start)
         s->src_ch[r] = (uint8_t)d.channels;
+        s->max_src_ch = std::max<uint32_t>(s->max_src_ch, d.channels);
     }
     s->has_biquad = any_biquad;
-    for (auto& c : s->classes) {
+    // slot rows, in the caller's order, then stably partitioned into classes
+    const uint32_t C = s->channels;
+    std::vector<rb_session::Slot> slots;
+    std::vector<uint32_t> rfrom, rto, rkey;
+    for (size_t i = 0; i < n; i++) {
+        const uint32_t r = s->pos[i], ci = chs[i];
+        auto add = [&](uint32_t ch0, uint32_t w, uint32_t cin) {
+            slots.push_back({r, (uint8_t)ch0, (uint8_t)w, (uint8_t)cin});
+            rfrom.push_back(from[i]), rto.push_back(to[i]);
+            rkey.push_back((key[i] & 0x700u) << 8 | cin | w << 2 | ch0 << 4);   // chain variant, slot
+        };
+        if (ci == 1 && C >= 2) add(0, 2, 1);
+        else
+            for (uint32_t c0 = 0, k = std::min(ci, C); c0 < k; c0 += 2) add(c0, std::min(2u, k - c0), std::min(2u, k - c0));
+        if (!(ci == 1 && C >= 2) && (ci > 2 || ci > C)) s->plain = false;
+    }
+    if (slots.size() > 0x7FFFFFFFull) return fail(RB_ERR_INVALID_ARGUMENT, "more than 2^31 slot rows");
+    const size_t nr = slots.size();
+    s->rows_of.assign(n, {});
+    std::vector<uint32_t> gslot;   // per partial row
+    uint32_t max_ci = 1;
+    for (const auto& cls : lanes::classes_by_ratio(rfrom.data(), rto.data(), rkey.data(), (uint32_t)nr)) {
+        rb_session::Class c;
+        const rb_session::Slot& s0 = slots[cls[0]];
+        const uint32_t src_key = rkey[cls[0]] >> 8;
+        c.first = (uint32_t)s->rows.size(), c.count = (uint32_t)cls.size(), c.ch_in = s0.ci, c.ch_out = s0.w;
+        c.front = (src_key & 0x400u) != 0;
+        c.has_biquad = (src_key & 0x100u) != 0 || c.front, c.has_pre = (src_key & 0x200u) != 0;
         c.ff2 = c.has_biquad;
-        for (uint32_t r = c.first; r < c.first + c.count; r++) c.ff2 = c.ff2 && row_ff2[r];
+        for (uint32_t q : cls) {
+            c.ff2 = c.ff2 && row_ff2[slots[q].src];
+            s->rows_of[slots[q].src].push_back((uint32_t)s->rows.size());
+            s->rows.push_back(slots[q]);
+        }
+        for (uint32_t g = 0; g < (c.count + 31) / 32; g++) gslot.push_back((uint32_t)s0.ch0 | (uint32_t)s0.w << 16);
+        max_ci = std::max<uint32_t>(max_ci, s0.ci);
+        s->classes.push_back(c);
     }
     RB_CUDA(cudaSetDevice(ctx->device));
-    const uint32_t C = s->channels;
-    s->stride = align_up((size_t)fifo_frames * C + 16, 32);
-    // every product below stays far inside 64 bits: n < 2^31, stride < 2^34 floats, max_block_frames < 2^32
-    if ((uint64_t)n * s->stride > (1ull << 40) || (uint64_t)max_block_frames * C * ((n + 31) / 32 + 1) > (1ull << 40))
+    s->n_groups = (uint32_t)gslot.size();
+#if defined(RB_SIMT_EMULATE)
+    s->emu_fast_tiles.assign(s->classes.size(), 0);
+#endif
+    s->stride = align_up((size_t)fifo_frames * max_ci + 16, 32);
+    // every product below stays far inside 64 bits: rows < 2^31, stride < 2^34 floats, max_block_frames < 2^32
+    if ((uint64_t)nr * s->stride > (1ull << 40) || (uint64_t)max_block_frames * C * (s->n_groups + 1) > (1ull << 40))
         return fail(RB_ERR_OUT_OF_MEMORY, "session of this size (sources x fifo_frames, or max_block_frames) exceeds 4 TB of device memory");
-    const size_t arena = n * s->stride * sizeof(float);
-    uint32_t n_groups = 0;   // partial rows: one per warp, every class rounds up on its own
-    for (const auto& c : s->classes) n_groups += (c.count + 31) / 32;
+    const size_t arena = nr * s->stride * sizeof(float);
     const uint64_t pstride = lanes::round_up_tile((uint64_t)max_block_frames * C);
     RB_CUDA(cudaMalloc(&s->d_fifo[0], arena));
     RB_CUDA(cudaMalloc(&s->d_fifo[1], arena));
-    RB_CUDA(cudaMalloc(&s->d_state, n * 4 * C * sizeof(float)));
+    RB_CUDA(cudaMalloc(&s->d_state, nr * 8 * sizeof(float)));
     RB_CUDA(cudaMalloc(&s->d_zeros, 256));
-    RB_CUDA(cudaMalloc(&s->d_partial, (size_t)n_groups * pstride * sizeof(float)));
+    RB_CUDA(cudaMalloc(&s->d_partial, (size_t)s->n_groups * pstride * sizeof(float)));
     RB_CUDA(cudaMalloc(&s->d_out, pstride * sizeof(float)));
-    RB_CUDA(cudaMalloc(&s->d_flags, n * sizeof(uint32_t)));
-    RB_CUDA(cudaMalloc(&s->d_rows, n * sizeof(lanes::Row)));
-    RB_CUDA(cudaMalloc(&s->d_u32, 2 * n * sizeof(uint32_t)));
-    RB_CUDA(cudaMalloc(&s->d_off, n * sizeof(uint64_t)));
-    RB_CUDA(cudaMallocHost(&s->h_off, n * sizeof(uint64_t)));
-    RB_CUDA(cudaMallocHost(&s->h_rows, n * sizeof(lanes::Row)));
-    RB_CUDA(cudaMallocHost(&s->h_u32, 2 * n * sizeof(uint32_t)));
+    RB_CUDA(cudaMalloc(&s->d_flags, nr * sizeof(uint32_t)));
+    RB_CUDA(cudaMalloc(&s->d_rows, nr * sizeof(lanes::Row)));
+    RB_CUDA(cudaMalloc(&s->d_u32, 2 * nr * sizeof(uint32_t)));
+    RB_CUDA(cudaMalloc(&s->d_slot, s->n_groups * sizeof(uint32_t)));
+    RB_CUDA(cudaMalloc(&s->d_jobs, nr * sizeof(rb_fifo_job)));
+    RB_CUDA(cudaMallocHost(&s->h_rows, nr * sizeof(lanes::Row)));
+    RB_CUDA(cudaMallocHost(&s->h_u32, 2 * nr * sizeof(uint32_t)));
+    RB_CUDA(cudaMallocHost(&s->h_jobs, nr * sizeof(rb_fifo_job)));
     RB_CUDA(cudaMallocHost(&s->h_out, pstride * sizeof(float)));
     RB_CUDA(cudaMemsetAsync(s->d_fifo[0], 0, arena, ctx->stream));
     RB_CUDA(cudaMemsetAsync(s->d_fifo[1], 0, arena, ctx->stream));
-    RB_CUDA(cudaMemsetAsync(s->d_state, 0, n * 4 * C * sizeof(float), ctx->stream));
+    RB_CUDA(cudaMemsetAsync(s->d_state, 0, nr * 8 * sizeof(float), ctx->stream));
     RB_CUDA(cudaMemsetAsync(s->d_zeros, 0, 256, ctx->stream));
-    RB_CUDA(cudaMemsetAsync(s->d_flags, 0, n * sizeof(uint32_t), ctx->stream));
+    RB_CUDA(cudaMemsetAsync(s->d_flags, 0, nr * sizeof(uint32_t), ctx->stream));
+    RB_CUDA(cudaMemcpyAsync(s->d_slot, gslot.data(), s->n_groups * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
     RB_CUDA(cudaStreamSynchronize(ctx->stream));
     *out = s.release();
     return RB_OK;
+}
+
+// The staging buffer of the pushes: every source's FIFO capacity in its own interleaving.
+static cudaError_t session_staging(rb_session* s) {
+    if (s->d_stage) return cudaSuccess;
+    return cudaMalloc(&s->d_stage, s->st.size() * (size_t)s->fifo_cap * s->max_src_ch * sizeof(float));
+}
+// Scatter jobs for `frames` new frames of source r (source order) at float offset `src` of the staging buffer, appended to
+// h_jobs from index j on; returns the new job count.
+static uint32_t session_jobs(rb_session* s, size_t r, uint64_t src, uint64_t frames, uint32_t j) {
+    for (uint32_t q : s->rows_of[r]) {
+        const rb_session::Slot& sl = s->rows[q];
+        s->h_jobs[j++] = rb_fifo_job{src, q, (uint32_t)frames, (uint32_t)s->st[r].fill(), s->src_ch[r], sl.ch0, sl.ci, 0};
+    }
+    return j;
 }
 
 extern "C" rb_status rb_session_push(rb_session* s, size_t stream, const float* pcm, uint64_t n_frames, int end_of_stream) {
@@ -1933,12 +2013,14 @@ extern "C" rb_status rb_session_push(rb_session* s, size_t stream, const float* 
     if (n_frames > s->fifo_cap - st.fill()) return fail(RB_ERR_BUFFER_TOO_SMALL, "the stream's FIFO is full: render first");
     RB_CUDA(cudaSetDevice(s->ctx->device));
     if (n_frames) {
-        // one stream: straight into the FIFO tail, classified in place (count = n for this stream only)
-        const uint32_t C = s->src_ch[stream];   // this source's interleaved channels
-        float* dst = s->d_fifo[s->cur] + stream * s->stride + st.fill() * C;
-        RB_CUDA(cudaMemcpyAsync(dst, pcm, n_frames * C * sizeof(float), cudaMemcpyHostToDevice, s->ctx->stream));
-        RB_CUDA(rb_lanes_classify_range(dst, n_frames * C, s->d_flags + stream, s->ctx->stream));
-        RB_CUDA(cudaStreamSynchronize(s->ctx->stream));   // the caller may reuse `pcm` as soon as we return
+        // one stream: into the staging buffer, scattered over the FIFOs of its rows
+        cudaStream_t stq = s->ctx->stream;
+        RB_CUDA(session_staging(s));
+        RB_CUDA(cudaMemcpyAsync(s->d_stage, pcm, n_frames * s->src_ch[stream] * sizeof(float), cudaMemcpyHostToDevice, stq));
+        const uint32_t n_jobs = session_jobs(s, stream, 0, n_frames, 0);
+        RB_CUDA(cudaMemcpyAsync(s->d_jobs, s->h_jobs, n_jobs * sizeof(rb_fifo_job), cudaMemcpyHostToDevice, stq));
+        RB_CUDA(rb_lanes_fifo_scatter(s->d_stage, s->d_jobs, n_jobs, s->d_fifo[s->cur], s->stride, s->d_flags, stq));
+        RB_CUDA(cudaStreamSynchronize(stq));   // the caller may reuse `pcm` as soon as we return
         st.pushed += n_frames;
     }
     if (end_of_stream) st.eof = true;
@@ -1958,19 +2040,18 @@ extern "C" rb_status rb_session_push_packed(rb_session* s, const float* pcm, con
     if (total && !pcm) return fail(RB_ERR_INVALID_ARGUMENT, "pcm is NULL");
     RB_CUDA(cudaSetDevice(s->ctx->device));
     if (total) {
-        if (!s->d_stage) RB_CUDA(cudaMalloc(&s->d_stage, ns * (size_t)s->fifo_cap * s->channels * sizeof(float)));
+        RB_CUDA(session_staging(s));
         uint64_t off = 0;   // floats: every source counts its own channels
+        uint32_t n_jobs = 0;
         for (size_t i = 0; i < ns; i++) {
             const size_t r = s->pos[i];
-            const uint32_t C = s->src_ch[r];
-            s->h_off[r] = off, s->h_u32[r] = (uint32_t)(n_frames[i] * C), s->h_u32[ns + r] = (uint32_t)(s->st[r].fill() * C);
-            off += n_frames[i] * C;
+            if (n_frames[i]) n_jobs = session_jobs(s, r, off, n_frames[i], n_jobs);
+            off += n_frames[i] * s->src_ch[r];
         }
         cudaStream_t stq = s->ctx->stream;
         RB_CUDA(cudaMemcpyAsync(s->d_stage, pcm, off * sizeof(float), cudaMemcpyHostToDevice, stq));
-        RB_CUDA(cudaMemcpyAsync(s->d_off, s->h_off, ns * sizeof(uint64_t), cudaMemcpyHostToDevice, stq));
-        RB_CUDA(cudaMemcpyAsync(s->d_u32, s->h_u32, 2 * ns * sizeof(uint32_t), cudaMemcpyHostToDevice, stq));
-        RB_CUDA(rb_lanes_fifo_append(s->d_stage, s->d_off, s->d_u32, s->d_u32 + ns, s->d_fifo[s->cur], s->stride, s->d_flags, (uint32_t)ns, stq));
+        RB_CUDA(cudaMemcpyAsync(s->d_jobs, s->h_jobs, n_jobs * sizeof(rb_fifo_job), cudaMemcpyHostToDevice, stq));
+        RB_CUDA(rb_lanes_fifo_scatter(s->d_stage, s->d_jobs, n_jobs, s->d_fifo[s->cur], s->stride, s->d_flags, stq));
         RB_CUDA(cudaStreamSynchronize(stq));
     }
     for (size_t i = 0; i < ns; i++) {
@@ -2007,6 +2088,8 @@ extern "C" rb_status rb_session_skip(rb_session* s, size_t stream) {
 extern "C" rb_status rb_session_set_amplify(rb_session* s, size_t stream, float factor) {
     if (!s) return fail(RB_ERR_INVALID_ARGUMENT, "session is NULL");
     if (stream >= s->st.size()) return fail(RB_ERR_INVALID_ARGUMENT, "stream index out of range");
+    if (s->pads[s->pos[stream]] && !std::isfinite(factor))
+        return fail(RB_ERR_UNSUPPORTED, "the source's conversion pads channels with 0.0: its gain behind the conversion stays finite");
     s->post[s->pos[stream]] = factor;
     s->has_post = true;   // sources without an AMPLIFY keep the factor 1.0: x * 1.0 is exact
     return RB_OK;
@@ -2020,8 +2103,9 @@ extern "C" rb_status rb_session_set_volume(rb_session* s, size_t stream, float f
         s->mid[r] = factor;   // the gain behind a filter in front is always applied
         return RB_OK;
     }
+    const uint32_t q = s->rows_of[r][0];
     for (const auto& c : s->classes)
-        if (r >= c.first && r < c.first + c.count && !c.has_pre)
+        if (q >= c.first && q < c.first + c.count && !c.has_pre)
             return fail(RB_ERR_STATE, "the source was declared without an AMPLIFY in front of the conversion (declare one with factor 1.0)");
     s->pre[r] = factor;
     return RB_OK;
@@ -2070,43 +2154,53 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
     if (!out_host) return fail(RB_ERR_INVALID_ARGUMENT, "out_host is NULL");
     RB_CUDA(cudaSetDevice(s->ctx->device));
     cudaStream_t stq = s->ctx->stream;
-    const size_t ns = s->st.size();
+    const size_t ns = s->st.size(), nr = s->rows.size();
     const uint32_t C = s->channels;
     std::vector<session::Part> parts(ns);
     std::vector<uint8_t> quiet(ns, 0);
     float* fifo = s->d_fifo[s->cur];
     for (size_t r = 0; r < ns; r++) {
-        const session::Part p = parts[r] = session::part_of(s->st[r], s->T, n);
-        lanes::Row& row = s->h_rows[r];
+        parts[r] = session::part_of(s->st[r], s->T, n);
+        if (!s->st[r].front && !(lanes::pre_gain_keeps_class(s->pre[r]) && lanes::pre_gain_keeps_class(s->vol_a[r]) && lanes::pre_gain_keeps_class(s->vol_b[r])))
+            quiet[r] = 1;   // its class runs the guarded tile in this block (or, DOWN, slow tiles)
+    }
+    for (size_t q = 0; q < nr; q++) {   // every row of a source renders the source's part: the rows stay in lock step
+        const size_t r = s->rows[q].src;
+        const session::Part& p = parts[r];
+        lanes::Row& row = s->h_rows[q];
         memset(&row, 0, sizeof(row));
-        row.in = fifo + r * s->stride, row.L = s->st[r].fill(), row.out_len = p.out_len, row.mix_start = p.mix_start;
-        row.n_int = p.n_int, row.o0 = p.o0, row.i0 = s->st[r].i0, row.state = s->d_state + 4 * C * r;
+        row.in = fifo + q * s->stride, row.L = s->st[r].fill(), row.out_len = p.out_len, row.mix_start = p.mix_start;
+        row.n_int = p.n_int, row.o0 = p.o0, row.i0 = s->st[r].i0, row.state = s->d_state + 8 * q;
         const float* co = &s->coef[5 * r];
         row.b0 = co[0], row.b1 = co[1], row.b2 = co[2], row.a1 = co[3], row.a2 = co[4], row.ffk = s->ffk[r];
         row.post = s->post[r], row.pre = s->pre[r], row.mid = s->mid[r];
-        row.flags = p.continues ? lanes::ROW_CONTINUES : 0u;
+        row.flags = (p.continues ? lanes::ROW_CONTINUES : 0u) | (quiet[r] ? lanes::ROW_FORCE_SLOW : 0u);
         row.f0 = s->st[r].fpos - s->st[r].i0, row.ga = s->vol_a[r], row.gb = s->vol_b[r];
-        if (!s->st[r].front && !(lanes::pre_gain_keeps_class(row.pre) && lanes::pre_gain_keeps_class(row.ga) && lanes::pre_gain_keeps_class(row.gb)))
-            row.flags |= lanes::ROW_FORCE_SLOW, quiet[r] = 1;   // its class runs the guarded tile in this block (or, DOWN, slow tiles)
     }
-    RB_CUDA(cudaMemcpyAsync(s->d_rows, s->h_rows, ns * sizeof(lanes::Row), cudaMemcpyHostToDevice, stq));
+    RB_CUDA(cudaMemcpyAsync(s->d_rows, s->h_rows, nr * sizeof(lanes::Row), cudaMemcpyHostToDevice, stq));
     const uint64_t pstride = lanes::round_up_tile((uint64_t)s->max_block * C);
-    const uint32_t n_groups_total = [&] { uint32_t g = 0; for (auto& c : s->classes) g += (c.count + 31) / 32; return g; }();
     // rows of the partial buffer are only written inside each warp's span: clear what this block may read
-    RB_CUDA(cudaMemsetAsync(s->d_partial, 0, (size_t)n_groups_total * pstride * sizeof(float), stq));
+    RB_CUDA(cudaMemsetAsync(s->d_partial, 0, (size_t)s->n_groups * pstride * sizeof(float), stq));
     uint32_t g0 = 0;
-    for (const auto& c : s->classes) {   // one launch per rate pair over its rows and its partial rows
+    for (const auto& c : s->classes) {   // one launch per class over its rows and its partial rows
         lanes::Args a{};
         a.rows = s->d_rows + c.first, a.n_rows = c.count, a.n_groups = (c.count + 31) / 32;
-        lanes::fill_ratio(a, s->st[c.first].from, s->st[c.first].to, C);
+        const session::Stream& s0 = s->st[s->rows[c.first].src];
+        lanes::fill_ratio(a, s0.from, s0.to, c.ch_out);
         a.mix_len = n, a.pstride = pstride;
         a.partial = s->d_partial + (size_t)g0 * pstride, a.zeros = s->d_zeros, a.unsafe = s->d_flags + c.first;
         bool guard = false;
-        for (uint32_t r = c.first; r < c.first + c.count; r++) guard = guard || quiet[r];
-        RB_CUDA(rb_lanes_launch_kernel(a, c.ch_in, C, c.has_biquad, c.ff2, s->has_post, c.has_pre, c.front, guard, stq));
+        for (uint32_t q = c.first; q < c.first + c.count; q++) guard = guard || quiet[s->rows[q].src];
+#if defined(RB_SIMT_EMULATE)
+        const uint64_t fast0 = simt::g_emu_count[0];
+#endif
+        RB_CUDA(rb_lanes_launch_kernel(a, c.ch_in, c.ch_out, c.has_biquad, c.ff2, s->has_post, c.has_pre, c.front, guard, stq));
+#if defined(RB_SIMT_EMULATE)
+        s->emu_fast_tiles[&c - s->classes.data()] += simt::g_emu_count[0] - fast0;
+#endif
         g0 += a.n_groups;
     }
-    RB_CUDA(rb_lanes_launch_sum(s->d_partial, n_groups_total, pstride, n * C, s->d_out, stq));
+    RB_CUDA(rb_lanes_launch_sum_slots(s->d_partial, s->d_slot, s->n_groups, pstride, n, C, s->d_out, stq));
     if (s->has_master) {
         // the block's active runs: frames some source covers.  A frame no source covers (a source declared to join later, the
         // others ended) is a gap: MixerSource::next() is None there, the chain is not pulled and the frame stays 0.0.
@@ -2148,10 +2242,13 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
         const uint64_t pulled = s->st[r].fpos - pulled_before;
         if (pulled >= 2) s->vol_a[r] = s->vol_b[r] = vol;
         else if (pulled == 1) s->vol_a[r] = s->vol_b[r], s->vol_b[r] = vol;
-        s->h_u32[r] = (uint32_t)(drop * s->src_ch[r]), s->h_u32[ns + r] = (uint32_t)((fill_before - drop) * s->src_ch[r]);   // floats
+        for (uint32_t q : s->rows_of[r]) {   // floats
+            const uint32_t ci = s->rows[q].ci;
+            s->h_u32[q] = (uint32_t)(drop * ci), s->h_u32[nr + q] = (uint32_t)((fill_before - drop) * ci);
+        }
     }
-    RB_CUDA_TX(cudaMemcpyAsync(s->d_u32, s->h_u32, 2 * ns * sizeof(uint32_t), cudaMemcpyHostToDevice, stq));
-    RB_CUDA_TX(rb_lanes_fifo_compact(fifo, s->d_fifo[s->cur ^ 1], s->stride, s->d_u32, s->d_u32 + ns, (uint32_t)ns, stq));
+    RB_CUDA_TX(cudaMemcpyAsync(s->d_u32, s->h_u32, 2 * nr * sizeof(uint32_t), cudaMemcpyHostToDevice, stq));
+    RB_CUDA_TX(rb_lanes_fifo_compact(fifo, s->d_fifo[s->cur ^ 1], s->stride, s->d_u32, s->d_u32 + nr, (uint32_t)nr, stq));
     s->cur ^= 1;
     RB_CUDA_TX(cudaMemcpyAsync(s->h_out, s->d_out, n * C * sizeof(float), cudaMemcpyDeviceToHost, stq));
     RB_CUDA_TX(cudaStreamSynchronize(stq));
@@ -2168,21 +2265,37 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
     return RB_OK;
 }
 
+#if defined(RB_SIMT_EMULATE)
+// CPU build only (not in the C ABI): fast tiles the emulator ran for each class of the session so far, in class order; returns
+// the number of classes.  Lets the tests show that no layout passes on slow tiles alone.
+extern "C" uint32_t rb_session_emu_fast_tiles(const rb_session* s, uint64_t* out, uint32_t cap) {
+    for (size_t k = 0; k < s->emu_fast_tiles.size() && k < cap; k++) out[k] = s->emu_fast_tiles[k];
+    return (uint32_t)s->emu_fast_tiles.size();
+}
+#endif
+
 // ---- block-to-block state as a blob ----
+// One record per slot row, in class order; the FIFO contents of every row follow the records.  A session whose every source is one
+// row carrying all of its channels (mono and stereo mixers, mono sources anywhere) writes version 5; any other layout writes
+// version 6, which adds one layout record per row between the records and the FIFO contents, so that a blob only restores a
+// session of the same layout.
 namespace {
 struct SessionBlobHeader {
-    uint32_t magic, version, n_streams, has_biquad, channels, pad_;
+    uint32_t magic, version, n_streams, has_biquad, channels, pad_;   // n_streams: rows
     uint64_t T;
 };
-struct SessionBlobStream {   // in class order (the same descriptors give the same order)
+struct SessionBlobStream {   // in class order (the same descriptors give the same order); the source's fields repeat on each of its rows
     uint64_t mix_start, pushed, out_done, i0;
     uint32_t from, to;
     uint32_t eof, unsafe, fill, filter_ahead;   // fill in frames; filter_ahead = fpos - i0 of a filter in front of the conversion
-    float state[8];                      // 4 per channel
+    float state[8];                      // 4 per channel of the row
     float vol_a, vol_b;                  // factor of the two frames in front of fpos (rb_session_set_volume)
     float vol, post;                     // the current factors: rb_session_set_volume / rb_session_set_amplify
     uint32_t held;                       // still waiting for rb_session_start / its predecessor (RB_SESSION_HELD)
-    int32_t follows;                     // class-order index of the source it is queued behind (rb_session_follow), -1: none
+    int32_t follows;                     // class-order index of the first row of the source it is queued behind (rb_session_follow), -1: none
+};
+struct SessionBlobSlot {     // version 6: the row's source (source order) and slot
+    uint32_t src, slot;      // slot = ch0 | w << 8 | ci << 16
 };
 // Behind the FIFO contents when the session has a master chain (header pad_ = 1); without one the blob ends with them.
 struct SessionBlobMaster {
@@ -2191,43 +2304,57 @@ struct SessionBlobMaster {
     float integ[RB_MAX_CHANNELS], peak[RB_MAX_CHANNELS];
 };
 constexpr uint32_t SESSION_MAGIC = 0x52425353u;   // "RBSS"
+SessionBlobSlot blob_slot(const rb_session::Slot& sl) { return {sl.src, (uint32_t)sl.ch0 | (uint32_t)sl.w << 8 | (uint32_t)sl.ci << 16}; }
+// the fields a source's rows share
+bool same_source_fields(const SessionBlobStream& a, const SessionBlobStream& b) {
+    return a.mix_start == b.mix_start && a.pushed == b.pushed && a.out_done == b.out_done && a.i0 == b.i0 && a.from == b.from && a.to == b.to &&
+           a.eof == b.eof && a.fill == b.fill && a.filter_ahead == b.filter_ahead && !memcmp(&a.vol_a, &b.vol_a, 4 * sizeof(float)) &&
+           a.held == b.held && a.follows == b.follows;
+}
 }  // namespace
 
 extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap, uint64_t* size) {
     if (!s || !size) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
-    const size_t ns = s->st.size();
-    uint64_t need = sizeof(SessionBlobHeader) + ns * sizeof(SessionBlobStream);
+    const size_t nr = s->rows.size();
+    const uint64_t n_slots = s->plain ? 0 : nr;
+    uint64_t need = sizeof(SessionBlobHeader) + nr * sizeof(SessionBlobStream) + n_slots * sizeof(SessionBlobSlot);
     const uint32_t C = s->channels;
-    for (size_t r = 0; r < ns; r++) need += s->st[r].fill() * s->src_ch[r] * sizeof(float);
+    for (size_t q = 0; q < nr; q++) need += s->st[s->rows[q].src].fill() * s->rows[q].ci * sizeof(float);
     if (s->has_master) need += sizeof(SessionBlobMaster);
     *size = need;
     if (!buf) return RB_OK;
     if (cap < need) return fail(RB_ERR_BUFFER_TOO_SMALL, "state buffer too small");
     RB_CUDA(cudaSetDevice(s->ctx->device));
-    std::vector<float> state(4 * C * ns);
-    std::vector<uint32_t> flags(ns);
-    RB_CUDA(cudaMemcpyAsync(state.data(), s->d_state, 4 * C * ns * sizeof(float), cudaMemcpyDeviceToHost, s->ctx->stream));
-    RB_CUDA(cudaMemcpyAsync(flags.data(), s->d_flags, ns * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->ctx->stream));
+    std::vector<float> state(8 * nr);
+    std::vector<uint32_t> flags(nr);
+    RB_CUDA(cudaMemcpyAsync(state.data(), s->d_state, 8 * nr * sizeof(float), cudaMemcpyDeviceToHost, s->ctx->stream));
+    RB_CUDA(cudaMemcpyAsync(flags.data(), s->d_flags, nr * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->ctx->stream));
     float mstate[2 * RB_MAX_CHANNELS] = {0};
     if (s->has_master)
         RB_CUDA(cudaMemcpyAsync(mstate, s->d_master[s->master_k], 2 * C * sizeof(float), cudaMemcpyDeviceToHost, s->ctx->stream));
     uint8_t* p = (uint8_t*)buf;
-    SessionBlobHeader h{SESSION_MAGIC, 5u, (uint32_t)ns, s->has_biquad ? 1u : 0u, C, s->has_master ? 1u : 0u, s->T};
+    SessionBlobHeader h{SESSION_MAGIC, s->plain ? 5u : 6u, (uint32_t)nr, s->has_biquad ? 1u : 0u, C, s->has_master ? 1u : 0u, s->T};
     memcpy(p, &h, sizeof(h)), p += sizeof(h);
     uint8_t* recs = p;
-    p += ns * sizeof(SessionBlobStream);
-    for (size_t r = 0; r < ns; r++) {
-        const uint64_t fill = s->st[r].fill() * s->src_ch[r];   // floats
-        if (fill) RB_CUDA(cudaMemcpyAsync(p, s->d_fifo[s->cur] + r * s->stride, fill * sizeof(float), cudaMemcpyDeviceToHost, s->ctx->stream));
+    p += nr * sizeof(SessionBlobStream);
+    for (size_t q = 0; q < n_slots; q++) {
+        const SessionBlobSlot sl = blob_slot(s->rows[q]);
+        memcpy(p, &sl, sizeof(sl)), p += sizeof(sl);
+    }
+    for (size_t q = 0; q < nr; q++) {
+        const uint64_t fill = s->st[s->rows[q].src].fill() * s->rows[q].ci;   // floats
+        if (fill) RB_CUDA(cudaMemcpyAsync(p, s->d_fifo[s->cur] + q * s->stride, fill * sizeof(float), cudaMemcpyDeviceToHost, s->ctx->stream));
         p += fill * sizeof(float);
     }
     RB_CUDA(cudaStreamSynchronize(s->ctx->stream));
-    for (size_t r = 0; r < ns; r++) {
+    for (size_t q = 0; q < nr; q++) {
+        const size_t r = s->rows[q].src;
         const session::Stream& st = s->st[r];
-        SessionBlobStream b{st.mix_start, st.pushed, st.out_done, st.i0, st.from, st.to, st.eof ? 1u : 0u, flags[r], (uint32_t)st.fill(), (uint32_t)(st.fpos - st.i0), {0}, s->vol_a[r], s->vol_b[r],
-                            st.front ? s->mid[r] : s->pre[r], s->post[r], st.held ? 1u : 0u, (int32_t)st.follows};
-        for (uint32_t k = 0; k < 4 * C; k++) b.state[k] = state[4 * C * r + k];
-        memcpy(recs + r * sizeof(b), &b, sizeof(b));
+        const int32_t follows = st.follows < 0 ? -1 : (int32_t)s->rows_of[(size_t)st.follows][0];
+        SessionBlobStream b{st.mix_start, st.pushed, st.out_done, st.i0, st.from, st.to, st.eof ? 1u : 0u, flags[q], (uint32_t)st.fill(), (uint32_t)(st.fpos - st.i0), {0}, s->vol_a[r], s->vol_b[r],
+                            st.front ? s->mid[r] : s->pre[r], s->post[r], st.held ? 1u : 0u, follows};
+        for (uint32_t k = 0; k < 8; k++) b.state[k] = state[8 * q + k];
+        memcpy(recs + q * sizeof(b), &b, sizeof(b));
     }
     if (s->has_master) {
         SessionBlobMaster m{};
@@ -2240,29 +2367,40 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
 
 extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64_t size) {
     if (!s || !buf) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
-    const size_t ns = s->st.size();
+    const size_t nr = s->rows.size();
+    const uint64_t n_slots = s->plain ? 0 : nr;
     const uint8_t* p = (const uint8_t*)buf;
     SessionBlobHeader h;
     if (size < sizeof(h)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
     memcpy(&h, p, sizeof(h)), p += sizeof(h);
     const uint32_t C = s->channels;
-    if (h.magic != SESSION_MAGIC || h.version != 5u) return fail(RB_ERR_INVALID_ARGUMENT, "not a session state blob");
-    if (h.n_streams != ns || h.has_biquad != (s->has_biquad ? 1u : 0u) || h.channels != C)
+    if (h.magic != SESSION_MAGIC || (h.version != 5u && h.version != 6u)) return fail(RB_ERR_INVALID_ARGUMENT, "not a session state blob");
+    if (h.version != (s->plain ? 5u : 6u) || h.n_streams != nr || h.has_biquad != (s->has_biquad ? 1u : 0u) || h.channels != C)
         return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session of another shape");
-    if (size < sizeof(h) + ns * sizeof(SessionBlobStream)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
-    std::vector<SessionBlobStream> recs(ns);
-    memcpy(recs.data(), p, ns * sizeof(SessionBlobStream)), p += ns * sizeof(SessionBlobStream);
-    uint64_t need = sizeof(h) + ns * sizeof(SessionBlobStream);
-    for (size_t r = 0; r < ns; r++) {
-        const SessionBlobStream& b = recs[r];
+    uint64_t need = sizeof(h) + nr * sizeof(SessionBlobStream) + n_slots * sizeof(SessionBlobSlot);
+    if (size < need) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
+    std::vector<SessionBlobStream> recs(nr);
+    memcpy(recs.data(), p, nr * sizeof(SessionBlobStream)), p += nr * sizeof(SessionBlobStream);
+    for (size_t q = 0; q < n_slots; q++) {
+        SessionBlobSlot sl, mine = blob_slot(s->rows[q]);
+        memcpy(&sl, p, sizeof(sl)), p += sizeof(sl);
+        if (memcmp(&sl, &mine, sizeof(sl)) != 0) return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session of another layout");
+    }
+    std::vector<uint8_t> first_row(nr, 0);
+    for (const auto& rows : s->rows_of) first_row[rows[0]] = 1;
+    for (size_t q = 0; q < nr; q++) {
+        const SessionBlobStream& b = recs[q];
+        const size_t r = s->rows[q].src;
         if (b.from != s->st[r].from || b.to != s->st[r].to) return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session of another shape");
         if (b.fill > s->fifo_cap || b.pushed - b.i0 != b.fill || (b.i0 & 3u) || b.filter_ahead > b.fill)
             return fail(RB_ERR_INVALID_ARGUMENT, "state blob: FIFO record out of range");
-        if (b.follows < -1 || (b.follows >= 0 && ((size_t)b.follows >= ns || (size_t)b.follows == r)))
+        if (b.follows < -1 || (b.follows >= 0 && ((size_t)b.follows >= nr || !first_row[(size_t)b.follows] || s->rows[(size_t)b.follows].src == r)))
             return fail(RB_ERR_INVALID_ARGUMENT, "state blob: queue record out of range");
         if (b.out_done > session::out_total(b.pushed, b.from, b.to))
             return fail(RB_ERR_INVALID_ARGUMENT, "state blob: more outputs rendered than the pushed input holds");
-        need += (uint64_t)b.fill * s->src_ch[r] * sizeof(float);
+        if (!same_source_fields(b, recs[s->rows_of[r][0]]))
+            return fail(RB_ERR_INVALID_ARGUMENT, "state blob: the rows of one source disagree");
+        need += (uint64_t)b.fill * s->rows[q].ci * sizeof(float);
     }
     if (h.pad_ != (s->has_master ? 1u : 0u)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session with another master chain");
     SessionBlobMaster m{};
@@ -2275,23 +2413,26 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
     }
     if (size < need) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
     RB_CUDA(cudaSetDevice(s->ctx->device));
-    std::vector<float> state(4 * C * ns);
-    std::vector<uint32_t> flags(ns);
-    for (size_t r = 0; r < ns; r++) {
-        const SessionBlobStream& b = recs[r];
+    std::vector<float> state(8 * nr);
+    std::vector<uint32_t> flags(nr);
+    for (size_t r = 0; r < s->st.size(); r++) {   // the source's fields, from its first row
+        const SessionBlobStream& b = recs[s->rows_of[r][0]];
         session::Stream& st = s->st[r];
         st.mix_start = b.mix_start, st.pushed = b.pushed, st.out_done = b.out_done, st.i0 = b.i0, st.eof = b.eof != 0, st.fpos = b.i0 + b.filter_ahead, s->vol_a[r] = b.vol_a, s->vol_b[r] = b.vol_b;
-        st.held = b.held != 0, st.follows = b.follows;
+        st.held = b.held != 0, st.follows = b.follows < 0 ? -1 : (int64_t)s->rows[(size_t)b.follows].src;
         (st.front ? s->mid[r] : s->pre[r]) = b.vol;
         if (b.post != s->post[r]) s->post[r] = b.post, s->has_post = true;
-        flags[r] = b.unsafe;
-        for (uint32_t k = 0; k < 4 * C; k++) state[4 * C * r + k] = b.state[k];
-        const size_t fill_floats = (size_t)b.fill * s->src_ch[r];
-        if (b.fill) RB_CUDA(cudaMemcpyAsync(s->d_fifo[s->cur] + r * s->stride, p, fill_floats * sizeof(float), cudaMemcpyHostToDevice, s->ctx->stream));
+    }
+    for (size_t q = 0; q < nr; q++) {
+        const SessionBlobStream& b = recs[q];
+        flags[q] = b.unsafe;
+        for (uint32_t k = 0; k < 8; k++) state[8 * q + k] = b.state[k];
+        const size_t fill_floats = (size_t)b.fill * s->rows[q].ci;
+        if (b.fill) RB_CUDA(cudaMemcpyAsync(s->d_fifo[s->cur] + q * s->stride, p, fill_floats * sizeof(float), cudaMemcpyHostToDevice, s->ctx->stream));
         p += fill_floats * sizeof(float);
     }
-    RB_CUDA(cudaMemcpyAsync(s->d_state, state.data(), 4 * C * ns * sizeof(float), cudaMemcpyHostToDevice, s->ctx->stream));
-    RB_CUDA(cudaMemcpyAsync(s->d_flags, flags.data(), ns * sizeof(uint32_t), cudaMemcpyHostToDevice, s->ctx->stream));
+    RB_CUDA(cudaMemcpyAsync(s->d_state, state.data(), 8 * nr * sizeof(float), cudaMemcpyHostToDevice, s->ctx->stream));
+    RB_CUDA(cudaMemcpyAsync(s->d_flags, flags.data(), nr * sizeof(uint32_t), cudaMemcpyHostToDevice, s->ctx->stream));
     float mstate[2 * RB_MAX_CHANNELS];
     if (s->has_master) {
         for (uint32_t c = 0; c < C; c++) mstate[c] = m.integ[c], mstate[C + c] = m.peak[c];

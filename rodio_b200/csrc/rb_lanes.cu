@@ -237,22 +237,37 @@ __global__ void __launch_bounds__(256) k_sum_groups(const float* __restrict__ pa
     }
 }
 
-// FIFO append + sticky classification, one CTA per stream
-__global__ void __launch_bounds__(128) k_fifo_append(const float* __restrict__ staging, const uint64_t* __restrict__ offset,
-                                                     const uint32_t* __restrict__ count, const uint32_t* __restrict__ fill,
-                                                     float* __restrict__ fifo, uint64_t stride, uint32_t* __restrict__ flags) {
-    const uint32_t r = blockIdx.x, n = count[r];
-    if (n == 0) return;
-    const float* __restrict__ src = staging + offset[r];
-    float* __restrict__ dst = fifo + (uint64_t)r * stride + fill[r];
+// out[f * C + j] = +0.0 + partial[g][f * w + j - o] for every group g (in order) whose slot [o, o + w) covers mixer channel j
+__global__ void __launch_bounds__(256) k_sum_slots(const float* __restrict__ partial, const uint32_t* __restrict__ slot, uint32_t n_groups,
+                                                   uint64_t pstride, uint64_t n_floats, uint32_t channels, float* __restrict__ out) {
+    for (uint64_t m = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; m < n_floats; m += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t f = m / channels;
+        const uint32_t j = (uint32_t)(m - f * channels);
+        float acc = 0.0f;
+        for (uint32_t g = 0; g < n_groups; g++) {
+            const uint32_t s = __ldg(slot + g), c = j - (s & 0xffffu), w = s >> 16;
+            if (c < w) acc = __fadd_rn(acc, partial[(uint64_t)g * pstride + f * w + c]);
+        }
+        out[m] = acc;
+    }
+}
+
+// FIFO scatter + sticky classification, one CTA per job (rb_lanes.h)
+__global__ void __launch_bounds__(128) k_fifo_scatter(const float* __restrict__ staging, const rb_fifo_job* __restrict__ jobs,
+                                                      float* __restrict__ fifo, uint64_t stride, uint32_t* __restrict__ flags) {
+    const rb_fifo_job j = jobs[blockIdx.x];
+    const uint32_t ci = j.ci, n = j.frames * ci;
+    const float* __restrict__ src = staging + j.src + j.ch0;
+    float* __restrict__ dst = fifo + (uint64_t)j.row * stride + (uint64_t)j.fill * ci;
     bool bad = false;
     for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
-        const float v = src[i];
+        const uint32_t f = ci == 1 ? i : i >> 1;
+        const float v = src[(uint64_t)f * j.src_ch + (i - f * ci)];
         const uint32_t u = __float_as_uint(v) & 0x7fffffffu;
         bad |= u != 0u && (u - 0x1c800000u) >= (0x5d800000u - 0x1c800000u);
         dst[i] = v;
     }
-    if (__syncthreads_or(bad ? 1 : 0) && threadIdx.x == 0) flags[r] = 1u;
+    if (__syncthreads_or(bad ? 1 : 0) && threadIdx.x == 0) flags[j.row] = 1u;
 }
 
 __global__ void __launch_bounds__(128) k_fifo_compact(const float* __restrict__ src, float* __restrict__ dst, uint64_t stride,
@@ -264,15 +279,6 @@ __global__ void __launch_bounds__(128) k_fifo_compact(const float* __restrict__ 
     for (uint32_t i = threadIdx.x; i < n4; i += blockDim.x)
         reinterpret_cast<float4*>(d)[i] = reinterpret_cast<const float4*>(s)[i];
     for (uint32_t i = n4 * 4 + threadIdx.x; i < n; i += blockDim.x) d[i] = s[i];
-}
-
-__global__ void __launch_bounds__(256) k_classify_range(const float* __restrict__ x, uint64_t n, uint32_t* __restrict__ flag) {
-    bool bad = false;
-    for (uint64_t i = threadIdx.x; i < n; i += blockDim.x) {
-        const uint32_t u = __float_as_uint(x[i]) & 0x7fffffffu;
-        bad |= u != 0u && (u - 0x1c800000u) >= (0x5d800000u - 0x1c800000u);
-    }
-    if (__syncthreads_or(bad ? 1 : 0) && threadIdx.x == 0) *flag = 1u;
 }
 
 template <int CI, int CO, bool HASB, bool FF2, int NPOST, bool PASS, bool PRE, bool FRONT = false, bool DOWN = false, bool GUARD = false>
@@ -375,16 +381,20 @@ cudaError_t rb_lanes_launch_sum(const float* d_partial, uint32_t n_groups, uint6
     return cudaGetLastError();
 }
 
-cudaError_t rb_lanes_fifo_append(const float* d_staging, const uint64_t* d_offset, const uint32_t* d_count, const uint32_t* d_fill,
-                                 float* d_fifo, uint64_t stride, uint32_t* d_flags, uint32_t n_streams, cudaStream_t st) {
-    if (n_streams == 0) return cudaSuccess;
-    k_fifo_append<<<n_streams, 128, 0, st>>>(d_staging, d_offset, d_count, d_fill, d_fifo, stride, d_flags);
+cudaError_t rb_lanes_launch_sum_slots(const float* d_partial, const uint32_t* d_slot, uint32_t n_groups, uint64_t pstride, uint64_t n_frames,
+                                      uint32_t channels, float* d_out, cudaStream_t st) {
+    const uint64_t n_floats = n_frames * channels;
+    if (n_floats == 0) return cudaSuccess;
+    uint64_t blocks = (n_floats + 255) / 256;
+    if (blocks > 132ull * 8) blocks = 132ull * 8;
+    k_sum_slots<<<(uint32_t)blocks, 256, 0, st>>>(d_partial, d_slot, n_groups, pstride, n_floats, channels, d_out);
     return cudaGetLastError();
 }
 
-cudaError_t rb_lanes_classify_range(const float* d_ptr, uint64_t n, uint32_t* d_flag, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_classify_range<<<1, 256, 0, st>>>(d_ptr, n, d_flag);
+cudaError_t rb_lanes_fifo_scatter(const float* d_staging, const rb_fifo_job* d_jobs, uint32_t n_jobs, float* d_fifo, uint64_t stride,
+                                  uint32_t* d_flags, cudaStream_t st) {
+    if (n_jobs == 0) return cudaSuccess;
+    k_fifo_scatter<<<n_jobs, 128, 0, st>>>(d_staging, d_jobs, d_fifo, stride, d_flags);
     return cudaGetLastError();
 }
 

@@ -81,15 +81,28 @@ cudaError_t rb_lerpmix_launch(const rb_lerpmix_args& a, cudaStream_t st);
 // ... and the ordered sum of n_groups partial rows (all classes) into d_out[0, n_floats).
 cudaError_t rb_lanes_launch_sum(const float* d_partial, uint32_t n_groups, uint64_t pstride, uint64_t n_floats, float* d_out,
                                 cudaStream_t st);
-// FIFO append: stream r receives count[r] frames, taken from staging + offset[r], behind its fill[r] frames in
-// fifo + r * stride; flags[r] becomes non-zero (and stays so) when a new frame lies outside the exact-reciprocal class.
-cudaError_t rb_lanes_fifo_append(const float* d_staging, const uint64_t* d_offset, const uint32_t* d_count, const uint32_t* d_fill,
-                                 float* d_fifo, uint64_t stride, uint32_t* d_flags, uint32_t n_streams, cudaStream_t st);
+// ---- the FIFOs and the mixer sum of the streaming sessions: one FIFO, one filter state and one input flag per SLOT ROW ----
+// A session source of CI channels feeds k = min(CI, mixer channels) of the mixer's channels; its rows carry channels
+// (2s, 2s + 1) as CI = CO = 2 rows and an odd last channel as a CI = CO = 1 row (a mono source in a wider mixer: one CI = 1,
+// CO = 2 row on channels 0 and 1).  A row's FIFO holds its `ci` channels interleaved.
+struct rb_fifo_job {          // one row of one push, 24 bytes
+    uint64_t src;             // float offset of the source's first new frame in the staging buffer
+    uint32_t row;             // FIFO (fifo + row * stride) and flag of the row
+    uint32_t frames, fill;    // new frames; frames already in the row's FIFO
+    uint8_t src_ch, ch0, ci;  // the source's interleaving; the first source channel the row carries, and how many (1 or 2)
+    uint8_t pad_;
+};
+// FIFO scatter: every job appends `frames` frames of channels [ch0, ch0 + ci) of its source behind the row's fill frames;
+// flags[row] becomes non-zero (and stays so) when one of them lies outside the exact-reciprocal class.  One CTA per job.
+cudaError_t rb_lanes_fifo_scatter(const float* d_staging, const rb_fifo_job* d_jobs, uint32_t n_jobs, float* d_fifo, uint64_t stride,
+                                  uint32_t* d_flags, cudaStream_t st);
 // FIFO compaction into the other arena: dst[r][0, keep[r]) = src[r][drop[r], drop[r] + keep[r]).
 cudaError_t rb_lanes_fifo_compact(const float* d_src, float* d_dst, uint64_t stride, const uint32_t* d_drop, const uint32_t* d_keep,
                                   uint32_t n_streams, cudaStream_t st);
-// Sticky classification of n freshly written floats at d_ptr: *d_flag = 1 when one lies outside the class.
-cudaError_t rb_lanes_classify_range(const float* d_ptr, uint64_t n, uint32_t* d_flag, cudaStream_t st);
+// The mixer sum over slots: group g's partial row holds frames of w = slot[g] >> 16 interleaved channels that land on mixer
+// channels [o, o + w), o = slot[g] & 0xffff.  out[f * C + j] = +0.0 + every partial row whose slot covers j, in group order.
+cudaError_t rb_lanes_launch_sum_slots(const float* d_partial, const uint32_t* d_slot, uint32_t n_groups, uint64_t pstride, uint64_t n_frames,
+                                      uint32_t channels, float* d_out, cudaStream_t st);
 // rows[r].flags takes the ROW_UNSAFE bit of stream_rows[row_stream[r]] (time-parallel plan: a stream is classified once, its
 // segment rows inherit the verdict); row_stream[r] == ~0u (padding) clears it.
 cudaError_t rb_lanes_spread_flags(lanes::Row* d_rows, uint32_t n_rows, const uint32_t* d_row_stream, const lanes::Row* d_stream_rows, cudaStream_t st);
