@@ -303,6 +303,7 @@ extern "C" {
                          fifo_frames: u32, max_block_frames: u32, out: *mut *mut rb_session) -> i32;
     fn rb_session_destroy(s: *mut rb_session) -> i32;
     fn rb_session_push_packed(s: *mut rb_session, pcm: *const f32, n_frames: *const u64, end_of_stream: *const u8) -> i32;
+    fn rb_session_push_silence(s: *mut rb_session, stream: usize, n_frames: u64) -> i32;
     fn rb_session_render(s: *mut rb_session, out: *mut f32, max_frames: u64, written: *mut u64, ended: *mut i32) -> i32;
     fn rb_session_follow(s: *mut rb_session, stream: usize, predecessor: usize) -> i32;
     fn rb_session_skip(s: *mut rb_session, stream: usize) -> i32;
@@ -328,6 +329,12 @@ pub struct GpuLiveMixer {
 }
 
 impl GpuLiveMixer {
+    /// `Player::pause` of input `stream` for `n_frames` frames: whole frames of 0.0 go to the mixer while the source (and any
+    /// fade or take at the front of its chain) is not pulled -- `Pausable` (src/source/pausable.rs).  Returns the rb_status.
+    pub fn push_silence(&mut self, stream: usize, n_frames: u64) -> i32 {
+        unsafe { rb_session_push_silence(self.session, stream, n_frames) }
+    }
+
     fn refill(&mut self) {
         // pull up to `pull_frames` samples from every live source -- packed: source 0's block, then source 1's, ...
         let mut pcm: Vec<f32> = Vec::with_capacity(self.inputs.len() * self.pull_frames);

@@ -6,7 +6,8 @@
  * (src/player.rs:120-128), so the user's filter and the Player's volume sit IN FRONT of the conversion to the mixer's format.
  * Here: two slots of one session, declared held; the second follows the first (rb_session_follow); set_volume changes the
  * AMPLIFY in front of the conversion for every frame pulled from then on (rb_session_set_volume); while paused the shim pushes
- * zero frames, like Pausable (src/source/pausable.rs:85-97).
+ * silence behind the source's chain (rb_session_push_silence), like Pausable (src/source/pausable.rs:85-97): a fade or take at
+ * the front of the chain stands still meanwhile.
  * Build:  gcc -std=c11 -Iinclude examples/live_player.c -Lrodio_b200 -l:librodio_b200.so -Wl,-rpath,$PWD/rodio_b200 -lm -o live_player
  * (needs a CUDA device at run time: rb_context_create fails loudly without one). */
 #include <math.h>
@@ -51,7 +52,7 @@ int main(void) {
     CHECK(rb_session_follow(player, 1, 0));  /* Player::append(song) */
 
     const int intro_blocks = 20, song_blocks = 30;   /* 10 ms each */
-    float pcm[441], zeros[441] = {0}, out[480];
+    float pcm[441], out[480];
     uint64_t total = 0, silent = 0;
     double peak_loud = 0.0, peak_quiet = 0.0;
     int ended = 0, sent_intro = 0, sent_song = 0;
@@ -66,7 +67,7 @@ int main(void) {
             sent_intro++;
             CHECK(rb_session_push(player, 0, pcm, 220, sent_intro == intro_blocks));
         } else if (paused) {
-            CHECK(rb_session_push(player, 1, zeros, 441, 0));    /* Pausable: frames of zeros, the source is not pulled */
+            CHECK(rb_session_push_silence(player, 1, 441));       /* Pausable: frames of zeros, the source is not pulled */
         } else if (sent_song < song_blocks) {
             for (int i = 0; i < 441; i++) pcm[i] = (float)(0.6 * sin(2 * M_PI * 440.0 * (sent_song * 441 + i) / SONG_RATE));
             sent_song++;

@@ -339,7 +339,15 @@ rb_status rb_batch_read_stream(rb_batch* b, size_t stream, float* out_host, uint
  * hands to Mixer::add or appends to a Player (src/player.rs:120-128): any SPEED (it only changes the rate pair), one filter
  * -- it then runs once per INPUT frame with coefficients for the rate its input reports (src/source/blt.rs to_applier) --,
  * one AMPLIFY in front of that filter and one behind it (src/source/amplify.rs:91-95; without a filter: one AMPLIFY).  One
- * filter per source, in front or behind.  Sources of different shapes may share a session (classes of their own); desc.n_samples / span_len are ignored,
+ * filter per source, in front or behind.  In front of all that the chain may begin with a PUSH PROGRAM: any number of LINEAR_RAMP
+ * (fade_in / fade_out), TAKE_DURATION and DISTORTION, with AMPLIFY and SPEED among them -- effects [0, p), p one past the last
+ * of the three.  Each sample they give is a function of its input sample and its index in the source, so they run as the PCM
+ * is pushed, at the rate the SPEEDs in front of each report; the AMPLIFYs behind the program stay the ones rb_session_set_volume
+ * and set_amplify change.  A take ends its source at its last frame (padded with 0.0 as take.rs:107-123 does): a push that
+ * reaches it is cut there, later pushes are dropped with RB_OK.  Behind a take rodio's conversion restarts every 32768 samples
+ * and never pulls the padding; sessions serve takes of one such run in whole frames, or sources at the mixer's rate whose
+ * channels pass through or restart on a frame boundary (RB_ERR_UNSUPPORTED otherwise), and no filter behind a take that ends
+ * inside a frame.  Sources of different shapes may share a session (classes of their own); desc.n_samples / span_len are ignored,
  * desc.mix_start is the mixer FRAME the source joins at.  Everything below counts frames; PCM is interleaved.
  * One caller per session; every call returns with the work done (the caller may reuse its buffers). */
 typedef struct rb_session rb_session;
@@ -358,6 +366,11 @@ rb_status rb_session_push(rb_session* s, size_t stream, const float* pcm, uint64
 /* The same for every source at once: pcm holds n_frames[0] frames of source 0, then n_frames[1] of source 1, ...;
  * end_of_stream may be NULL.  One host->device copy and one kernel for the whole session. */
 rb_status rb_session_push_packed(rb_session* s, const float* pcm, const uint64_t* n_frames, const uint8_t* end_of_stream);
+/* Player::pause / play for one source: n_frames frames of literal 0.0 behind its push program, what Pausable hands out while
+ * paused (src/source/pausable.rs:85-97) -- the program in front is not pulled, so fades and takes stand still.  They take FIFO
+ * room like a push (RB_ERR_BUFFER_TOO_SMALL).  RB_ERR_UNSUPPORTED for a source with a filter in front of the conversion:
+ * rodio freezes that filter while paused, the session would run it over the zeros. */
+rb_status rb_session_push_silence(rb_session* s, size_t stream, uint64_t n_frames);
 /* Mixer::add for a source declared with RB_SESSION_HELD: it joins at the mixer frame rendered next (sources join on a frame
  * boundary, src/mixer.rs:175-183).  While no source is playing the session renders nothing and its timeline stands still,
  * as MixerSource::next() returns None (src/mixer.rs:129-135); `ended` stays 0 as long as a held source may still come. */
@@ -395,7 +408,8 @@ rb_status rb_session_render(rb_session* s, float* out_host, uint64_t max_frames,
  * rb_batch_get_state / rb_batch_set_state of SURVEY.md 8b): a session of the same shape restored from it, on any
  * context, continues bit-identically.  buf == NULL: only *size is returned.  One record per slot row; a session whose every
  * source is one row carrying all of its channels (mono and stereo mixers, mono sources in any mixer) writes version 5, any
- * other layout version 6 with a layout record per row.  A blob of another shape, layout or master chain: RB_ERR_INVALID_ARGUMENT. */
+ * other layout version 6 with a layout record per row; a session with push programs writes version 7, which adds the program
+ * frames each source has consumed and the programs.  A blob of another shape, layout, master chain or program: RB_ERR_INVALID_ARGUMENT. */
 rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap, uint64_t* size);
 rb_status rb_session_set_state(rb_session* s, const void* buf, uint64_t size);
 

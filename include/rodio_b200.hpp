@@ -382,6 +382,8 @@ class LiveMixer {
     void push(size_t i, const std::vector<Sample>& pcm, bool end_of_stream = false) {
         check(rb_session_push(h_, i, pcm.data(), pcm.size() / src_channels_.at(i), end_of_stream ? 1 : 0), "rb_session_push");
     }
+    // Player::pause for n_frames frames: whole frames of 0.0 behind the source's push program, which is not pulled meanwhile
+    void push_silence(size_t i, uint64_t n_frames) { check(rb_session_push_silence(h_, i, n_frames), "rb_session_push_silence"); }
     // Mixer::add (mixer.rs:58-66) for a source that was declared held (its desc().mix_start == RB_SESSION_HELD)
     void add(size_t i) { check(rb_session_start(h_, i), "rb_session_start"); }
     // queue a held source behind another one: Player::append / queue.rs:128-192

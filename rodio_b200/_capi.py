@@ -101,6 +101,7 @@ SYMBOLS = {
     "rb_session_destroy": (C.c_int32, [C.c_void_p]),
     "rb_session_push": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint64, C.c_int]),
     "rb_session_push_packed": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rb_session_push_silence": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_uint64]),
     "rb_session_start": (C.c_int32, [C.c_void_p, C.c_size_t]),
     "rb_session_follow": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_size_t]),
     "rb_session_skip": (C.c_int32, [C.c_void_p, C.c_size_t]),

@@ -581,6 +581,32 @@ static rb_status plan_varying(PlanStream& ps, std::vector<SeqSeg> segs, size_t f
     return RB_OK;
 }
 
+// The closed-form adapters DISTORTION, LINEAR_RAMP and TAKE_DURATION on a stream of `c` channels whose input reports `rate`:
+// kind and parameters of the node.  A take's count is the samples it emits before `remaining < dps` (0 when dps is 0); the batch
+// planner bounds it by the input's length, the sessions' push programs by the frames pushed.
+static rb_status plan_pointwise(const rb_effect& e, uint32_t rate, uint32_t c, rb_node_dev& d) {
+    switch (e.kind) {
+        case RB_FX_DISTORTION:
+            if (!(e.f32[1] >= 0.0f)) return fail(RB_ERR_INVALID_ARGUMENT, "distortion: clamp(-t, t) panics for t < 0 or NaN");
+            d.kind = RB_N_DISTORT, d.p.dist.gain = e.f32[0], d.p.dist.threshold = e.f32[1];
+            return RB_OK;
+        case RB_FX_LINEAR_RAMP:
+            if (e.ns[0] == 0) return fail(RB_ERR_INVALID_ARGUMENT, "linear_gain_ramp: duration must be greater than zero");
+            d.kind = RB_N_RAMP;
+            d.p.ramp.total_ns = e.ns[0], d.p.ramp.dt_ns = 1000000000ull / rate;   // linear_ramp.rs:97-99
+            d.p.ramp.start = e.f32[0], d.p.ramp.end = e.f32[1], d.p.ramp.clamp_end = e.u32[0] ? 1u : 0u;
+            return RB_OK;
+        default: {   // RB_FX_TAKE_DURATION
+            const uint64_t dps = 1000000000ull / ((uint64_t)rate * c);                   // take.rs:65-69
+            d.kind = RB_N_TAKE;
+            d.p.take.total_ns = e.ns[0], d.p.take.dps_ns = dps, d.p.take.count = dps ? e.ns[0] / dps : 0;
+            d.p.take.total_ms_f = (float)(e.ns[0] / 1000000ull);
+            d.p.take.fadeout = e.u32[0] ? 1u : 0u;
+            return RB_OK;
+        }
+    }
+}
+
 static rb_status plan_stream(PlanStream& ps, uint16_t mixer_ch, uint32_t mixer_rate, std::vector<PlanStream>* all = nullptr, size_t self = 0) {
     const rb_stream_desc& d = ps.desc;
     ps.consumed = d.mix_start == RB_MIX_START_CONSUMED;
@@ -779,28 +805,20 @@ static rb_status plan_stream(PlanStream& ps, uint16_t mixer_ch, uint32_t mixer_r
                 cv_last = (buffer_spans && span != 0 && n >= c) ? (int64_t)((n / c - 1) * co) : -1;
                 break;
             }
-            case RB_FX_DISTORTION: {
-                if (!(e.f32[1] >= 0.0f)) return fail(RB_ERR_INVALID_ARGUMENT, "distortion: clamp(-t, t) panics for t < 0 or NaN");
-                nd.d.kind = RB_N_DISTORT, nd.d.p.dist.gain = e.f32[0], nd.d.p.dist.threshold = e.f32[1];
-                break;
-            }
+            case RB_FX_DISTORTION:
             case RB_FX_LINEAR_RAMP: {
-                if (e.ns[0] == 0) return fail(RB_ERR_INVALID_ARGUMENT, "linear_gain_ramp: duration must be greater than zero");
-                nd.d.kind = RB_N_RAMP;
-                nd.d.p.ramp.total_ns = e.ns[0], nd.d.p.ramp.dt_ns = 1000000000ull / rate;   // linear_ramp.rs:97-99
-                nd.d.p.ramp.start = e.f32[0], nd.d.p.ramp.end = e.f32[1], nd.d.p.ramp.clamp_end = e.u32[0] ? 1u : 0u;
+                rb_status s = plan_pointwise(e, rate, c, nd.d);
+                if (s != RB_OK) return s;
                 break;
             }
             case RB_FX_TAKE_DURATION: {
-                const uint64_t dps = 1000000000ull / ((uint64_t)rate * c);                   // take.rs:65-69
-                uint64_t take_n = dps ? e.ns[0] / dps : n;        // samples emitted before `remaining < dps`
+                plan_pointwise(e, rate, c, nd.d);
+                const uint64_t dps = nd.d.p.take.dps_ns;
+                uint64_t take_n = dps ? nd.d.p.take.count : n;        // samples emitted before `remaining < dps`
                 uint64_t count = std::min<uint64_t>(n, take_n);
                 uint64_t pad = 0;
                 if (dps && take_n <= n && count % c) pad = c - count % c;   // duration expired first: pad the frame
-                nd.d.kind = RB_N_TAKE;
-                nd.d.p.take.total_ns = e.ns[0], nd.d.p.take.dps_ns = dps, nd.d.p.take.count = count;
-                nd.d.p.take.total_ms_f = (float)(e.ns[0] / 1000000ull);
-                nd.d.p.take.fadeout = e.u32[0] ? 1u : 0u;
+                nd.d.p.take.count = count;
                 nd.d.n_out = count + pad;
                 // a take that does not cut (it outlasts its input) hands the padding of a take INSIDE it on: the span it reports is still
                 // the inner one's, so a UniformSourceIterator behind it stops in front of that padding all the same
@@ -1737,7 +1755,7 @@ struct rb_session {
     uint32_t mixer_rate = 0;
     uint32_t channels = 1;        // of the mixer (1 .. RB_MAX_CHANNELS)
     std::vector<uint8_t> src_ch;  // per source (source order): its own channel count
-    std::vector<uint8_t> pads;    // per source: its conversion pads channels with 0.0
+    std::vector<uint8_t> pads;    // per source: its conversion pads channels with 0.0 (1), its take pads its last frame (2)
     bool has_biquad = false, has_post = false;
     // Sources may have different rates (each at or below the mixer's): one kernel launch per reduced rate pair.  All
     // per-source arrays below are in SOURCE ORDER (stable partition by rate pair, channels and chain variant); pos[] maps the
@@ -1788,6 +1806,16 @@ struct rb_session {
     int master_k = 0;
     rb_master_run* d_master_runs = nullptr;    // the block's active runs, [n_streams]
     rb_master_run* h_master_runs = nullptr;
+    // push programs (rb_lanes.h: rb_prog_op): the closed-form adapters a source's chain begins with, applied by the scatter of
+    // every push.  Per source (source order): its ops, the frames that went through them, and where its take ends the source.
+    bool has_prog = false;
+    std::vector<rb_prog_op> prog_ops;
+    std::vector<uint32_t> prog_op0, prog_n;
+    std::vector<uint64_t> prog_pos;
+    std::vector<uint64_t> prog_end;            // frames: the take's count padded to whole frames; ~0: no take
+    std::vector<uint8_t> no_silence;           // a take in front of a resampling conversion: rb_session_push_silence refused
+    rb_prog_op* d_prog = nullptr;
+    rb_fifo_prog_job *d_pjobs = nullptr, *h_pjobs = nullptr;
 #if defined(RB_SIMT_EMULATE)
     std::vector<uint64_t> emu_fast_tiles;      // CPU build: fast tiles the emulator ran per class (rb_session_emu_fast_tiles)
 #endif
@@ -1800,6 +1828,7 @@ extern "C" rb_status rb_session_destroy(rb_session* s) {
     cudaFree(s->d_out), cudaFree(s->d_flags), cudaFree(s->d_rows), cudaFree(s->d_u32), cudaFree(s->d_slot), cudaFree(s->d_jobs), cudaFree(s->d_stage);
     cudaFreeHost(s->h_rows), cudaFreeHost(s->h_u32), cudaFreeHost(s->h_jobs), cudaFreeHost(s->h_out);
     cudaFree(s->d_master[0]), cudaFree(s->d_master[1]), cudaFree(s->d_master_runs), cudaFreeHost(s->h_master_runs);
+    cudaFree(s->d_prog), cudaFree(s->d_pjobs), cudaFreeHost(s->h_pjobs);
     delete s;
     return RB_OK;
 }
@@ -1821,6 +1850,9 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
     std::vector<uint32_t> from(n), to(n), chs(n), first_fx(n), key(n);
     std::vector<float> pre_of(n, 1.0f), mid_of(n, 1.0f);
     std::vector<uint32_t> front_fx(n, 0xFFFFFFFFu), front_rate(n, 0);
+    std::vector<std::vector<rb_prog_op>> progs(n);
+    std::vector<uint64_t> take_n(n, ~0ull);   // samples the source's takes let through
+    std::vector<uint8_t> no_silence(n, 0);
     for (size_t i = 0; i < n; i++) {
         const rb_stream_desc& d = descs[i];
         const std::string where = "stream " + std::to_string(i) + ": ";
@@ -1830,10 +1862,51 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
         if (mixer_channels == 1 && d.channels != 1) return fail(RB_ERR_UNSUPPORTED, where + "a mono mixer takes mono sources");
         chs[i] = d.channels;
         if (d.n_effects && !d.effects) return fail(RB_ERR_INVALID_ARGUMENT, where + "effects is NULL");
+        // The push program: effects [0, p), p one past the last LINEAR_RAMP / TAKE_DURATION / DISTORTION in front of everything
+        // else.  No state depends on the signal there: every output sample is a function of its input sample and its index in
+        // the source, so the scatter of each push applies them.  Each one sees the rate the SPEEDs in front of it report.
+        uint32_t p = 0, rate = d.sample_rate;
+        for (uint32_t k = 0; k < d.n_effects; k++) {
+            const uint32_t kd = d.effects[k].kind;
+            if (kd == RB_FX_LINEAR_RAMP || kd == RB_FX_TAKE_DURATION || kd == RB_FX_DISTORTION) p = k + 1;
+            else if (kd != RB_FX_AMPLIFY && kd != RB_FX_SPEED) break;
+        }
+        bool take_open = false;   // ops behind a take that ends inside a frame see its 0.0 padding
+        for (uint32_t k = 0; k < p; k++) {
+            const rb_effect& e = d.effects[k];
+            if (e.kind == RB_FX_SPEED) {
+                rate = rb_speed_sample_rate(rate, e.f32[0]);
+                if (rate == 0) return fail(RB_ERR_INVALID_ARGUMENT, where + "speed: zero sample rate");
+                continue;
+            }
+            rb_prog_op op;
+            memset(&op, 0, sizeof(op));
+            if (e.kind == RB_FX_AMPLIFY) {
+                op.kind = RB_N_AMPLIFY, op.p.amp = e.f32[0];
+            } else {
+                rb_node_dev nd;
+                memset(&nd, 0, sizeof(nd));
+                rb_status st = plan_pointwise(e, rate, d.channels, nd);
+                if (st != RB_OK) return st;
+                if (nd.kind == RB_N_TAKE) {
+                    if (nd.p.take.dps_ns == 0) return fail(RB_ERR_INVALID_ARGUMENT, where + "take_duration: the duration per sample is 0");
+                    take_n[i] = std::min(take_n[i], nd.p.take.count);
+                }
+                op.kind = nd.kind;
+                memcpy(&op.p, &nd.p, sizeof(op.p));
+            }
+            // the padding is 0.0: every factor behind it keeps it a zero, as rodio never pulls it (it only completes the frame)
+            if (take_open && !(op.kind == RB_N_AMPLIFY ? std::isfinite(op.p.amp)
+                               : op.kind == RB_N_DISTORT ? std::isfinite(op.p.dist.gain)
+                               : op.kind == RB_N_RAMP ? std::isfinite(op.p.ramp.start) && std::isfinite(op.p.ramp.end) : true))
+                return fail(RB_ERR_UNSUPPORTED, where + "a non-finite factor behind a take that ends inside a frame (rodio never pulls its padding)");
+            if (op.kind == RB_N_TAKE && op.p.take.count % d.channels) take_open = true;
+            progs[i].push_back(op);
+        }
         // Source::speed in front of the conversion only changes the rate the source reports (src/source/speed.rs:130-133);
         // one Source::amplify there -- `source.amplify(v)` handed to Mixer::add -- scales every frame before it is interpolated
         // (src/source/amplify.rs:91-95).  The two commute: one touches the samples, the other the reported rate.
-        uint32_t k0 = 0, rate = d.sample_rate;
+        uint32_t k0 = p;
         bool has_pre = false, has_mid = false, front = false;
         // A filter there as well -- `source.low_pass(f)` handed to the mixer, or appended to a Player, which keeps its volume
         // behind it (src/player.rs:120-128) -- runs at the rate its input reports at that point (src/source/blt.rs:
@@ -1854,6 +1927,23 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
         from[i] = rate / g, to[i] = mixer_rate / g;
         const bool filtered = k0 + 1 < d.n_effects && (d.effects[k0 + 1].kind == RB_FX_LOW_PASS || d.effects[k0 + 1].kind == RB_FX_HIGH_PASS);
         if (front && filtered) return fail(RB_ERR_UNSUPPORTED, where + "one filter per source: in front of the conversion or behind it");
+        if (take_n[i] != ~0ull) {
+            // Behind a take the mixer's conversion re-bootstraps every min(samples left, 32768) samples (src/source/uniform.rs:50-68,
+            // take.rs:180-196) and never pulls the padding of the take's last frame.  A session converts the source as one run, with
+            // the padding: the same samples when the take is one run of whole frames, or when the conversion keeps no state across a
+            // restart -- the source's own rate, and channels passed through or restarted on a frame boundary.
+            const uint64_t C_in = d.channels;
+            const bool whole = take_n[i] % C_in == 0;
+            const bool one_run = whole && take_n[i] <= RB_UNIFORM_SPAN_CAP;
+            const bool stateless = from[i] == to[i] && (take_n[i] <= RB_UNIFORM_SPAN_CAP || C_in == 1 || C_in == mixer_channels || RB_UNIFORM_SPAN_CAP % C_in == 0);
+            if (!one_run && !stateless)
+                return fail(RB_ERR_UNSUPPORTED, where + "take_duration: the mixer's conversion restarts every 32768 samples behind a take; "
+                                                        "sessions serve longer takes (or takes that end inside a frame) at the mixer's rate only");
+            if (!whole && (front || filtered))
+                return fail(RB_ERR_UNSUPPORTED, where + "a take that ends inside a frame pads it with 0.0, which a filter would see (rodio never pulls it)");
+            // Pausable passes the take's span on: the conversion then counts the pause's zeros against the take and restarts early
+            if (from[i] != to[i]) no_silence[i] = 1;
+        }
         // filtered / unfiltered sources, sources with / without a gain in front and sources whose filter sits in front are
         // classes of their own (a filter in front always applies the gains around it: no class of its own for those)
         key[i] = d.channels | (filtered ? 0x100u : 0u) | (has_pre && !front ? 0x200u : 0u) | (front ? 0x400u : 0u);
@@ -1867,6 +1957,7 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
     // pass 2: chains, in source order
     s->st.resize(n), s->coef.assign(5 * n, 0.0f), s->ffk.assign(n, 0.0f), s->post.assign(n, 1.0f), s->pre.assign(n, 1.0f), s->mid.assign(n, 1.0f), s->src_ch.assign(n, 1);
     s->vol_a.assign(n, 1.0f), s->vol_b.assign(n, 1.0f), s->pads.assign(n, 0);
+    s->prog_op0.assign(n, 0), s->prog_n.assign(n, 0), s->prog_pos.assign(n, 0), s->prog_end.assign(n, ~0ull), s->no_silence.assign(n, 0);
     bool any_biquad = false;
     std::vector<uint8_t> row_ff2(n, 1);
     for (size_t r = 0; r < n; r++) {
@@ -1901,6 +1992,11 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
         if (k != d.n_effects) return fail(RB_ERR_UNSUPPORTED, where + "chain shape: [SPEED | AMPLIFY | one filter] UNIFORM [LOW_PASS | HIGH_PASS] [AMPLIFY]");
         // Channels the conversion pads get no row: their 0.0 must stay a zero behind the filter and the gain
         s->pads[r] = mixer_channels > (d.channels == 1 ? 2u : d.channels);
+        if (take_n[i] != ~0ull && take_n[i] % d.channels) {   // ... and so must the padding of a take's last frame, behind every gain
+            s->pads[r] |= 2;
+            if (!std::isfinite(pre_of[i]) || !std::isfinite(mid_of[i]))
+                return fail(RB_ERR_UNSUPPORTED, where + "a take that ends inside a frame, behind a non-finite gain (rodio never pulls its padding)");
+        }
         if (s->pads[r]) {
             const float* co = &s->coef[5 * r];
             bool finite = std::isfinite(s->post[r]);
@@ -1912,7 +2008,14 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
         if (d.mix_start == RB_SESSION_HELD) s->st[r].held = true, s->st[r].mix_start = 0;   // Mixer::add comes later (rb_session_start)
         s->src_ch[r] = (uint8_t)d.channels;
         s->max_src_ch = std::max<uint32_t>(s->max_src_ch, d.channels);
+        s->prog_op0[r] = (uint32_t)s->prog_ops.size(), s->prog_n[r] = (uint32_t)progs[i].size(), s->no_silence[r] = no_silence[i];
+        s->prog_ops.insert(s->prog_ops.end(), progs[i].begin(), progs[i].end());
+        if (take_n[i] != ~0ull) {   // the take's last frame, padded: the source ends there
+            s->prog_end[r] = (take_n[i] + d.channels - 1) / d.channels;
+            if (s->prog_end[r] == 0) s->st[r].eof = true;
+        }
     }
+    s->has_prog = !s->prog_ops.empty();
     s->has_biquad = any_biquad;
     // slot rows, in the caller's order, then stably partitioned into classes
     const uint32_t C = s->channels;
@@ -1984,6 +2087,12 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
     RB_CUDA(cudaMemsetAsync(s->d_zeros, 0, 256, ctx->stream));
     RB_CUDA(cudaMemsetAsync(s->d_flags, 0, nr * sizeof(uint32_t), ctx->stream));
     RB_CUDA(cudaMemcpyAsync(s->d_slot, gslot.data(), s->n_groups * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    if (s->has_prog) {   // the program table goes to the device once; every push of such a session carries program jobs
+        RB_CUDA(cudaMalloc(&s->d_prog, s->prog_ops.size() * sizeof(rb_prog_op)));
+        RB_CUDA(cudaMalloc(&s->d_pjobs, nr * sizeof(rb_fifo_prog_job)));
+        RB_CUDA(cudaMallocHost(&s->h_pjobs, nr * sizeof(rb_fifo_prog_job)));
+        RB_CUDA(cudaMemcpyAsync(s->d_prog, s->prog_ops.data(), s->prog_ops.size() * sizeof(rb_prog_op), cudaMemcpyHostToDevice, ctx->stream));
+    }
     RB_CUDA(cudaStreamSynchronize(ctx->stream));
     *out = s.release();
     return RB_OK;
@@ -1999,9 +2108,32 @@ static cudaError_t session_staging(rb_session* s) {
 static uint32_t session_jobs(rb_session* s, size_t r, uint64_t src, uint64_t frames, uint32_t j) {
     for (uint32_t q : s->rows_of[r]) {
         const rb_session::Slot& sl = s->rows[q];
-        s->h_jobs[j++] = rb_fifo_job{src, q, (uint32_t)frames, (uint32_t)s->st[r].fill(), s->src_ch[r], sl.ch0, sl.ci, 0};
+        const rb_fifo_job job{src, q, (uint32_t)frames, (uint32_t)s->st[r].fill(), s->src_ch[r], sl.ch0, sl.ci, 0};
+        if (s->has_prog) s->h_pjobs[j++] = rb_fifo_prog_job{job, s->prog_pos[r], s->prog_op0[r], s->prog_n[r]};
+        else s->h_jobs[j++] = job;
     }
     return j;
+}
+static cudaError_t session_scatter(rb_session* s, uint32_t n_jobs, cudaStream_t stq) {
+    cudaError_t e;
+    if (s->has_prog) {
+        e = cudaMemcpyAsync(s->d_pjobs, s->h_pjobs, n_jobs * sizeof(rb_fifo_prog_job), cudaMemcpyHostToDevice, stq);
+        return e != cudaSuccess ? e : rb_lanes_fifo_scatter_prog(s->d_stage, s->d_pjobs, n_jobs, s->d_prog, s->d_fifo[s->cur], s->stride, s->d_flags, stq);
+    }
+    e = cudaMemcpyAsync(s->d_jobs, s->h_jobs, n_jobs * sizeof(rb_fifo_job), cudaMemcpyHostToDevice, stq);
+    return e != cudaSuccess ? e : rb_lanes_fifo_scatter(s->d_stage, s->d_jobs, n_jobs, s->d_fifo[s->cur], s->stride, s->d_flags, stq);
+}
+// A take has ended source r (source order): rodio stops pulling its input, so whatever is pushed later is dropped.
+static bool session_take_ended(const rb_session* s, size_t r) { return s->prog_pos[r] >= s->prog_end[r]; }
+// Frames of a push of n frames into source r that its take lets through (all of them without a take).
+static uint64_t session_take_room(const rb_session* s, size_t r, uint64_t n) {
+    return std::min(n, s->prog_end[r] - std::min(s->prog_end[r], s->prog_pos[r]));
+}
+// After `frames` frames went into source r: its program index advances; the take's last frame ends the source.
+static void session_pushed(rb_session* s, size_t r, uint64_t frames) {
+    s->st[r].pushed += frames;
+    s->prog_pos[r] += frames;
+    if (session_take_ended(s, r)) s->st[r].eof = true;
 }
 
 extern "C" rb_status rb_session_push(rb_session* s, size_t stream, const float* pcm, uint64_t n_frames, int end_of_stream) {
@@ -2009,21 +2141,43 @@ extern "C" rb_status rb_session_push(rb_session* s, size_t stream, const float* 
     if (stream >= s->st.size()) return fail(RB_ERR_INVALID_ARGUMENT, "stream index out of range");
     stream = s->pos[stream];   // class order from here on
     session::Stream& st = s->st[stream];
-    if (st.eof) return n_frames ? fail(RB_ERR_STATE, "push after end_of_stream") : RB_OK;
-    if (n_frames > s->fifo_cap - st.fill()) return fail(RB_ERR_BUFFER_TOO_SMALL, "the stream's FIFO is full: render first");
+    if (st.eof) return n_frames && !session_take_ended(s, stream) ? fail(RB_ERR_STATE, "push after end_of_stream") : RB_OK;
+    const uint64_t take = session_take_room(s, stream, n_frames);
+    if (take > s->fifo_cap - st.fill()) return fail(RB_ERR_BUFFER_TOO_SMALL, "the stream's FIFO is full: render first");
     RB_CUDA(cudaSetDevice(s->ctx->device));
-    if (n_frames) {
+    if (take) {
         // one stream: into the staging buffer, scattered over the FIFOs of its rows
         cudaStream_t stq = s->ctx->stream;
         RB_CUDA(session_staging(s));
-        RB_CUDA(cudaMemcpyAsync(s->d_stage, pcm, n_frames * s->src_ch[stream] * sizeof(float), cudaMemcpyHostToDevice, stq));
-        const uint32_t n_jobs = session_jobs(s, stream, 0, n_frames, 0);
-        RB_CUDA(cudaMemcpyAsync(s->d_jobs, s->h_jobs, n_jobs * sizeof(rb_fifo_job), cudaMemcpyHostToDevice, stq));
-        RB_CUDA(rb_lanes_fifo_scatter(s->d_stage, s->d_jobs, n_jobs, s->d_fifo[s->cur], s->stride, s->d_flags, stq));
+        RB_CUDA(cudaMemcpyAsync(s->d_stage, pcm, take * s->src_ch[stream] * sizeof(float), cudaMemcpyHostToDevice, stq));
+        RB_CUDA(session_scatter(s, session_jobs(s, stream, 0, take, 0), stq));
         RB_CUDA(cudaStreamSynchronize(stq));   // the caller may reuse `pcm` as soon as we return
-        st.pushed += n_frames;
+        session_pushed(s, stream, take);
     }
     if (end_of_stream) st.eof = true;
+    return RB_OK;
+}
+
+extern "C" rb_status rb_session_push_silence(rb_session* s, size_t stream, uint64_t n_frames) {
+    if (!s) return fail(RB_ERR_INVALID_ARGUMENT, "session is NULL");
+    if (stream >= s->st.size()) return fail(RB_ERR_INVALID_ARGUMENT, "stream index out of range");
+    const size_t r = s->pos[stream];
+    session::Stream& st = s->st[r];
+    if (st.front)   // rodio does not pull that filter while paused; the render would run it over the zeros
+        return fail(RB_ERR_UNSUPPORTED, "silence into a source with a filter in front of the conversion");
+    if (s->no_silence[r] && !st.eof)   // rodio's conversion counts the zeros against the take's span and restarts early
+        return fail(RB_ERR_UNSUPPORTED, "silence into a source whose take is in front of a resampling conversion");
+    if (st.eof) return n_frames && !session_take_ended(s, r) ? fail(RB_ERR_STATE, "silence after end_of_stream") : RB_OK;
+    if (n_frames > s->fifo_cap - st.fill()) return fail(RB_ERR_BUFFER_TOO_SMALL, "the stream's FIFO is full: render first");
+    if (n_frames == 0) return RB_OK;
+    RB_CUDA(cudaSetDevice(s->ctx->device));
+    cudaStream_t stq = s->ctx->stream;
+    for (uint32_t q : s->rows_of[r]) {   // literal +0.0 behind the program: inside the exact-reciprocal class, no flag to set
+        const uint32_t ci = s->rows[q].ci;
+        RB_CUDA(cudaMemsetAsync(s->d_fifo[s->cur] + q * s->stride + st.fill() * ci, 0, n_frames * ci * sizeof(float), stq));
+    }
+    RB_CUDA(cudaStreamSynchronize(stq));
+    st.pushed += n_frames;   // the program's index stands still
     return RB_OK;
 }
 
@@ -2031,31 +2185,39 @@ extern "C" rb_status rb_session_push_packed(rb_session* s, const float* pcm, con
     if (!s || !n_frames) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
     const size_t ns = s->st.size();
     uint64_t total = 0;
+    std::vector<uint64_t> take(ns);   // per caller's index: the frames the source's take lets through
     for (size_t i = 0; i < ns; i++) {   // i: the caller's index, pos[i]: class order
         const session::Stream& st = s->st[s->pos[i]];
-        if (st.eof && n_frames[i]) return fail(RB_ERR_STATE, "stream " + std::to_string(i) + ": push after end_of_stream");
-        if (n_frames[i] > s->fifo_cap - st.fill()) return fail(RB_ERR_BUFFER_TOO_SMALL, "stream " + std::to_string(i) + ": FIFO full, render first");
+        if (st.eof && n_frames[i] && !session_take_ended(s, s->pos[i])) return fail(RB_ERR_STATE, "stream " + std::to_string(i) + ": push after end_of_stream");
+        take[i] = st.eof ? 0 : session_take_room(s, s->pos[i], n_frames[i]);
+        if (take[i] > s->fifo_cap - st.fill()) return fail(RB_ERR_BUFFER_TOO_SMALL, "stream " + std::to_string(i) + ": FIFO full, render first");
         total += n_frames[i];
     }
     if (total && !pcm) return fail(RB_ERR_INVALID_ARGUMENT, "pcm is NULL");
     RB_CUDA(cudaSetDevice(s->ctx->device));
     if (total) {
         RB_CUDA(session_staging(s));
-        uint64_t off = 0;   // floats: every source counts its own channels
+        cudaStream_t stq = s->ctx->stream;
+        // Only the frames kept go to the staging buffer, which holds a full FIFO per source: what a take cuts off (or drops
+        // after it has ended) is not bounded by the FIFO.  Without such a cut the packed buffer is staged as it is, in one copy.
+        bool cut = false;
+        for (size_t i = 0; i < ns; i++) cut = cut || take[i] != n_frames[i];
+        uint64_t off = 0, staged = 0;   // floats, in the caller's buffer and in the staging buffer: every source counts its own channels
         uint32_t n_jobs = 0;
         for (size_t i = 0; i < ns; i++) {
             const size_t r = s->pos[i];
-            if (n_frames[i]) n_jobs = session_jobs(s, r, off, n_frames[i], n_jobs);
-            off += n_frames[i] * s->src_ch[r];
+            if (take[i]) {
+                n_jobs = session_jobs(s, r, staged, take[i], n_jobs);
+                if (cut) RB_CUDA(cudaMemcpyAsync(s->d_stage + staged, pcm + off, take[i] * s->src_ch[r] * sizeof(float), cudaMemcpyHostToDevice, stq));
+            }
+            off += n_frames[i] * s->src_ch[r], staged += take[i] * s->src_ch[r];
         }
-        cudaStream_t stq = s->ctx->stream;
-        RB_CUDA(cudaMemcpyAsync(s->d_stage, pcm, off * sizeof(float), cudaMemcpyHostToDevice, stq));
-        RB_CUDA(cudaMemcpyAsync(s->d_jobs, s->h_jobs, n_jobs * sizeof(rb_fifo_job), cudaMemcpyHostToDevice, stq));
-        RB_CUDA(rb_lanes_fifo_scatter(s->d_stage, s->d_jobs, n_jobs, s->d_fifo[s->cur], s->stride, s->d_flags, stq));
+        if (!cut) RB_CUDA(cudaMemcpyAsync(s->d_stage, pcm, off * sizeof(float), cudaMemcpyHostToDevice, stq));
+        RB_CUDA(session_scatter(s, n_jobs, stq));
         RB_CUDA(cudaStreamSynchronize(stq));
     }
     for (size_t i = 0; i < ns; i++) {
-        s->st[s->pos[i]].pushed += n_frames[i];
+        session_pushed(s, s->pos[i], take[i]);
         if (end_of_stream && end_of_stream[i]) s->st[s->pos[i]].eof = true;
     }
     return RB_OK;
@@ -2099,6 +2261,8 @@ extern "C" rb_status rb_session_set_volume(rb_session* s, size_t stream, float f
     if (!s) return fail(RB_ERR_INVALID_ARGUMENT, "session is NULL");
     if (stream >= s->st.size()) return fail(RB_ERR_INVALID_ARGUMENT, "stream index out of range");
     const size_t r = s->pos[stream];
+    if ((s->pads[r] & 2) && !std::isfinite(factor))
+        return fail(RB_ERR_UNSUPPORTED, "the source's take ends inside a frame: the gain in front of the conversion stays finite");
     if (s->st[r].front) {
         s->mid[r] = factor;   // the gain behind a filter in front is always applied
         return RB_OK;
@@ -2303,7 +2467,14 @@ struct SessionBlobMaster {
     uint32_t channels;
     float integ[RB_MAX_CHANNELS], peak[RB_MAX_CHANNELS];
 };
+// Version 7 (a session with push programs): the layout records of every row as in version 6, then one record per source (source
+// order) and the program table, then the FIFO contents.  A blob only restores a session with the same programs.
+struct SessionBlobProg {
+    uint64_t frames;                     // frames of the source that went through its program
+    uint32_t op0, n_ops;
+};
 constexpr uint32_t SESSION_MAGIC = 0x52425353u;   // "RBSS"
+uint32_t blob_version(const rb_session* s) { return s->has_prog ? 7u : s->plain ? 5u : 6u; }
 SessionBlobSlot blob_slot(const rb_session::Slot& sl) { return {sl.src, (uint32_t)sl.ch0 | (uint32_t)sl.w << 8 | (uint32_t)sl.ci << 16}; }
 // the fields a source's rows share
 bool same_source_fields(const SessionBlobStream& a, const SessionBlobStream& b) {
@@ -2315,9 +2486,10 @@ bool same_source_fields(const SessionBlobStream& a, const SessionBlobStream& b) 
 
 extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap, uint64_t* size) {
     if (!s || !size) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
-    const size_t nr = s->rows.size();
-    const uint64_t n_slots = s->plain ? 0 : nr;
-    uint64_t need = sizeof(SessionBlobHeader) + nr * sizeof(SessionBlobStream) + n_slots * sizeof(SessionBlobSlot);
+    const size_t nr = s->rows.size(), ns = s->st.size();
+    const uint64_t n_slots = blob_version(s) == 5u ? 0 : nr;
+    const uint64_t prog_bytes = s->has_prog ? ns * sizeof(SessionBlobProg) + s->prog_ops.size() * sizeof(rb_prog_op) : 0;
+    uint64_t need = sizeof(SessionBlobHeader) + nr * sizeof(SessionBlobStream) + n_slots * sizeof(SessionBlobSlot) + prog_bytes;
     const uint32_t C = s->channels;
     for (size_t q = 0; q < nr; q++) need += s->st[s->rows[q].src].fill() * s->rows[q].ci * sizeof(float);
     if (s->has_master) need += sizeof(SessionBlobMaster);
@@ -2333,13 +2505,20 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
     if (s->has_master)
         RB_CUDA(cudaMemcpyAsync(mstate, s->d_master[s->master_k], 2 * C * sizeof(float), cudaMemcpyDeviceToHost, s->ctx->stream));
     uint8_t* p = (uint8_t*)buf;
-    SessionBlobHeader h{SESSION_MAGIC, s->plain ? 5u : 6u, (uint32_t)nr, s->has_biquad ? 1u : 0u, C, s->has_master ? 1u : 0u, s->T};
+    SessionBlobHeader h{SESSION_MAGIC, blob_version(s), (uint32_t)nr, s->has_biquad ? 1u : 0u, C, s->has_master ? 1u : 0u, s->T};
     memcpy(p, &h, sizeof(h)), p += sizeof(h);
     uint8_t* recs = p;
     p += nr * sizeof(SessionBlobStream);
     for (size_t q = 0; q < n_slots; q++) {
         const SessionBlobSlot sl = blob_slot(s->rows[q]);
         memcpy(p, &sl, sizeof(sl)), p += sizeof(sl);
+    }
+    if (s->has_prog) {
+        for (size_t r = 0; r < ns; r++) {
+            const SessionBlobProg b{s->prog_pos[r], s->prog_op0[r], s->prog_n[r]};
+            memcpy(p, &b, sizeof(b)), p += sizeof(b);
+        }
+        memcpy(p, s->prog_ops.data(), s->prog_ops.size() * sizeof(rb_prog_op)), p += s->prog_ops.size() * sizeof(rb_prog_op);
     }
     for (size_t q = 0; q < nr; q++) {
         const uint64_t fill = s->st[s->rows[q].src].fill() * s->rows[q].ci;   // floats
@@ -2367,17 +2546,18 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
 
 extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64_t size) {
     if (!s || !buf) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
-    const size_t nr = s->rows.size();
-    const uint64_t n_slots = s->plain ? 0 : nr;
+    const size_t nr = s->rows.size(), ns = s->st.size();
+    const uint64_t n_slots = blob_version(s) == 5u ? 0 : nr;
+    const uint64_t prog_bytes = s->has_prog ? ns * sizeof(SessionBlobProg) + s->prog_ops.size() * sizeof(rb_prog_op) : 0;
     const uint8_t* p = (const uint8_t*)buf;
     SessionBlobHeader h;
     if (size < sizeof(h)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
     memcpy(&h, p, sizeof(h)), p += sizeof(h);
     const uint32_t C = s->channels;
-    if (h.magic != SESSION_MAGIC || (h.version != 5u && h.version != 6u)) return fail(RB_ERR_INVALID_ARGUMENT, "not a session state blob");
-    if (h.version != (s->plain ? 5u : 6u) || h.n_streams != nr || h.has_biquad != (s->has_biquad ? 1u : 0u) || h.channels != C)
+    if (h.magic != SESSION_MAGIC || h.version < 5u || h.version > 7u) return fail(RB_ERR_INVALID_ARGUMENT, "not a session state blob");
+    if (h.version != blob_version(s) || h.n_streams != nr || h.has_biquad != (s->has_biquad ? 1u : 0u) || h.channels != C)
         return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session of another shape");
-    uint64_t need = sizeof(h) + nr * sizeof(SessionBlobStream) + n_slots * sizeof(SessionBlobSlot);
+    uint64_t need = sizeof(h) + nr * sizeof(SessionBlobStream) + n_slots * sizeof(SessionBlobSlot) + prog_bytes;
     if (size < need) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
     std::vector<SessionBlobStream> recs(nr);
     memcpy(recs.data(), p, nr * sizeof(SessionBlobStream)), p += nr * sizeof(SessionBlobStream);
@@ -2385,6 +2565,19 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
         SessionBlobSlot sl, mine = blob_slot(s->rows[q]);
         memcpy(&sl, p, sizeof(sl)), p += sizeof(sl);
         if (memcmp(&sl, &mine, sizeof(sl)) != 0) return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session of another layout");
+    }
+    std::vector<uint64_t> prog_pos(ns, 0);
+    if (s->has_prog) {
+        for (size_t r = 0; r < ns; r++) {
+            SessionBlobProg b;
+            memcpy(&b, p, sizeof(b)), p += sizeof(b);
+            if (b.op0 != s->prog_op0[r] || b.n_ops != s->prog_n[r] || b.frames > s->prog_end[r])
+                return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session with other push programs");
+            prog_pos[r] = b.frames;
+        }
+        if (memcmp(p, s->prog_ops.data(), s->prog_ops.size() * sizeof(rb_prog_op)) != 0)
+            return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session with other push programs");
+        p += s->prog_ops.size() * sizeof(rb_prog_op);
     }
     std::vector<uint8_t> first_row(nr, 0);
     for (const auto& rows : s->rows_of) first_row[rows[0]] = 1;
@@ -2440,5 +2633,6 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
     }
     RB_CUDA(cudaStreamSynchronize(s->ctx->stream));
     s->T = h.T;
+    if (s->has_prog) s->prog_pos = prog_pos;
     return RB_OK;
 }

@@ -27,6 +27,40 @@ __device__ __forceinline__ float lerp_f(float first, float second, float num_f, 
     return add(first, divf(mul(sub(second, first), num_f), den_f));
 }
 
+// std::time::Duration::as_secs_f32 of `ns` nanoseconds: (secs as f32) + (nanos as f32) / 1e9
+__device__ __forceinline__ float duration_secs_f32(uint64_t ns) {
+    const uint64_t secs = ns / 1000000000ull;
+    const uint32_t nanos = (uint32_t)(ns - secs * 1000000000ull);
+    return add(__ull2float_rn(secs), divf(__uint2float_rn(nanos), 1000000000.0f));
+}
+
+// The closed-form per-sample adapters: k_distort / k_ramp / k_take (rb_kernels.cu) and the push programs of the sessions
+// (k_fifo_scatter, rb_lanes.cu) run these bodies.  rb_session_host.h restates them for the CPU build in the same order.
+// Distortion -- src/source/distortion.rs:66-72 : (x * gain).clamp(-t, t)   (f32::clamp: NaN passes through)
+__device__ __forceinline__ float distort_sample(float x, float g, float t) {
+    float v = mul(x, g);
+    if (v < -t) v = -t;
+    if (v > t) v = t;
+    return v;
+}
+// LinearGainRamp -- src/source/linear_ramp.rs:79-104: the factor of a sample whose frame has seen `elapsed` ns
+// (elapsed = frame * floor(1e9 / rate): the elapsed time advances once per frame while the ramp is running).
+// after: the factor once the ramp is over (end with clamp_end, else 1.0); total_f = duration_secs_f32(total).
+__device__ __forceinline__ float ramp_factor(uint64_t elapsed, uint64_t total, float start, float end, float after, float total_f) {
+    float factor = after;
+    if (elapsed < total) {
+        const float p = divf(duration_secs_f32(elapsed), total_f);
+        factor = add(mul(start, sub(1.0f, p)), mul(end, p));
+    }
+    return factor;
+}
+// TakeDuration's fade-out filter -- src/source/take.rs:34-41 on input sample `o` (o < count):
+// sample * (remaining.as_millis() as f32) / (total.as_millis() as f32)
+__device__ __forceinline__ float take_fade(float v, uint64_t o, uint64_t total, uint64_t dps, float total_ms) {
+    const uint64_t remaining_ms = (total - o * dps) / 1000000ull;
+    return divf(mul(v, __ull2float_rn(remaining_ms)), total_ms);
+}
+
 // src/source/blt.rs:558-560 : b0*x + b1*x1 + b2*x2 - a1*y1 - a2*y2, strictly left to right
 __device__ __forceinline__ float biquad(float b0, float b1, float b2, float a1, float a2, float x, float x1, float x2,
                                         float y1, float y2) {

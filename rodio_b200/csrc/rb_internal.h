@@ -56,6 +56,11 @@ struct rb_uniform_params {
 // Limiter coefficients (src/source/limit.rs:94-130, :854-988); attack / release for the rate the limiter was built at.
 struct rb_lim_params { float threshold, knee, inv_knee_8, attack, release; };
 
+// The closed-form per-sample adapters (rb_dsp.cuh): the general kernels and the push programs of the sessions share them.
+struct rb_dist_params { float gain, threshold; };
+struct rb_ramp_params { uint64_t total_ns, dt_ns; float start, end; uint32_t clamp_end; };
+struct rb_take_params { uint64_t total_ns, dps_ns, count; float total_ms_f; uint32_t fadeout; };
+
 // One adapter applied to one stream, as the device sees it.  POD, 16-byte aligned.
 struct alignas(16) rb_node_dev {
     const void* src;       // f32 except for RB_N_CONVERT
@@ -79,9 +84,9 @@ struct alignas(16) rb_node_dev {
         struct { float target, max_gain, floor, attack, release; } agc;
         rb_lim_params lim;
         struct { float vol[RB_MAX_CHANNELS]; } cv;
-        struct { float gain, threshold; } dist;
-        struct { uint64_t total_ns, dt_ns; float start, end; uint32_t clamp_end; } ramp;
-        struct { uint64_t total_ns, dps_ns, count; float total_ms_f; uint32_t fadeout; } take;
+        rb_dist_params dist;
+        rb_ramp_params ramp;
+        rb_take_params take;
         struct { float step; uint32_t fn; } sig;
         struct { uint64_t n2; } mix2;
         struct { uint64_t at, n; } pause;

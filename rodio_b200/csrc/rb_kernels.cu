@@ -180,19 +180,7 @@ __global__ void __launch_bounds__(TPB) k_distort(const rb_node_dev* __restrict__
     const rb_node_dev& nd = nodes[blockIdx.x];
     const float* __restrict__ x = (const float*)nd.src;
     const float g = nd.p.dist.gain, t = nd.p.dist.threshold;
-    for_each_out(nd, [&](uint64_t o) {
-        float v = mul(x[o], g);
-        if (v < -t) v = -t;
-        if (v > t) v = t;
-        nd.dst[o] = v;
-    });
-}
-
-// std::time::Duration::as_secs_f32 of `ns` nanoseconds: (secs as f32) + (nanos as f32) / 1e9
-__device__ __forceinline__ float duration_secs_f32(uint64_t ns) {
-    const uint64_t secs = ns / 1000000000ull;
-    const uint32_t nanos = (uint32_t)(ns - secs * 1000000000ull);
-    return add(__ull2float_rn(secs), divf(__uint2float_rn(nanos), 1000000000.0f));
+    for_each_out(nd, [&](uint64_t o) { nd.dst[o] = distort_sample(x[o], g, t); });
 }
 
 // LinearGainRamp / fade_in / fade_out — src/source/linear_ramp.rs:79-104.  Frame f sees
@@ -206,12 +194,7 @@ __global__ void __launch_bounds__(TPB) k_ramp(const rb_node_dev* __restrict__ no
     const float total_f = duration_secs_f32(total);
     const uint32_t C = nd.c_in;
     for_each_out(nd, [&](uint64_t o) {
-        const uint64_t elapsed = (o / C) * dt;
-        float factor = after;
-        if (elapsed < total) {
-            const float p = divf(duration_secs_f32(elapsed), total_f);
-            factor = add(mul(start, sub(1.0f, p)), mul(end, p));
-        }
+        const float factor = ramp_factor((o / C) * dt, total, start, end, after, total_f);
         nd.dst[o] = mul(x[o], factor);
     });
 }
@@ -228,10 +211,7 @@ __global__ void __launch_bounds__(TPB) k_take(const rb_node_dev* __restrict__ no
         float v = 0.0f;                                   // Sample::EQUILIBRIUM padding
         if (o < count) {
             v = x[o];
-            if (fade) {
-                const uint64_t remaining_ms = (total - o * dps) / 1000000ull;
-                v = divf(mul(v, __ull2float_rn(remaining_ms)), total_ms);
-            }
+            if (fade) v = take_fade(v, o, total, dps, total_ms);
         }
         nd.dst[o] = v;
     });

@@ -11,6 +11,7 @@
 #include "rb_lanes.h"
 #include "rb_lanes_plan.h"
 #include "rb_duo_core.h"
+#include "rb_dsp.cuh"
 
 namespace {
 
@@ -252,17 +253,55 @@ __global__ void __launch_bounds__(256) k_sum_slots(const float* __restrict__ par
     }
 }
 
-// FIFO scatter + sticky classification, one CTA per job (rb_lanes.h)
-__global__ void __launch_bounds__(128) k_fifo_scatter(const float* __restrict__ staging, const rb_fifo_job* __restrict__ jobs,
-                                                      float* __restrict__ fifo, uint64_t stride, uint32_t* __restrict__ flags) {
-    const rb_fifo_job j = jobs[blockIdx.x];
+// A push program on sample n of its source (rb_lanes.h: rb_prog_op), in chain order.  Past a take's count the sample is the
+// take's Sample::EQUILIBRIUM padding, which the ops behind it still see.
+__device__ __forceinline__ float run_prog(float v, uint64_t n, uint32_t C, const rb_prog_op* __restrict__ ops, uint32_t n_ops) {
+    for (uint32_t k = 0; k < n_ops; k++) {
+        const rb_prog_op& op = ops[k];
+        switch (op.kind) {
+            case RB_N_AMPLIFY: v = rbd::mul(v, op.p.amp); break;
+            case RB_N_DISTORT: v = rbd::distort_sample(v, op.p.dist.gain, op.p.dist.threshold); break;
+            case RB_N_RAMP: {
+                const rb_ramp_params& r = op.p.ramp;
+                const float factor = rbd::ramp_factor((n / C) * r.dt_ns, r.total_ns, r.start, r.end, r.clamp_end ? r.end : 1.0f,
+                                                      rbd::duration_secs_f32(r.total_ns));
+                v = rbd::mul(v, factor);
+                break;
+            }
+            default: {   // RB_N_TAKE
+                const rb_take_params& t = op.p.take;
+                if (n < t.count) {
+                    if (t.fadeout) v = rbd::take_fade(v, n, t.total_ns, t.dps_ns, t.total_ms_f);
+                } else {
+                    v = 0.0f;
+                }
+            }
+        }
+    }
+    return v;
+}
+
+// FIFO scatter + sticky classification, one CTA per job (rb_lanes.h).  PROG: the jobs are rb_fifo_prog_job and every sample
+// runs through its source's push program first.
+template <bool PROG>
+__global__ void __launch_bounds__(128) k_fifo_scatter(const float* __restrict__ staging, const void* __restrict__ jobs_,
+                                                      float* __restrict__ fifo, uint64_t stride, uint32_t* __restrict__ flags,
+                                                      const rb_prog_op* __restrict__ ops) {
+    const rb_fifo_job j = PROG ? static_cast<const rb_fifo_prog_job*>(jobs_)[blockIdx.x].j : static_cast<const rb_fifo_job*>(jobs_)[blockIdx.x];
     const uint32_t ci = j.ci, n = j.frames * ci;
     const float* __restrict__ src = staging + j.src + j.ch0;
     float* __restrict__ dst = fifo + (uint64_t)j.row * stride + (uint64_t)j.fill * ci;
+    uint64_t base = 0;
+    uint32_t op0 = 0, n_ops = 0;
+    if (PROG) {
+        const rb_fifo_prog_job& pj = static_cast<const rb_fifo_prog_job*>(jobs_)[blockIdx.x];
+        base = pj.base, op0 = pj.op0, n_ops = pj.n_ops;
+    }
     bool bad = false;
     for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
         const uint32_t f = ci == 1 ? i : i >> 1;
-        const float v = src[(uint64_t)f * j.src_ch + (i - f * ci)];
+        float v = src[(uint64_t)f * j.src_ch + (i - f * ci)];
+        if (PROG) v = run_prog(v, (base + f) * j.src_ch + j.ch0 + (i - f * ci), j.src_ch, ops + op0, n_ops);
         const uint32_t u = __float_as_uint(v) & 0x7fffffffu;
         bad |= u != 0u && (u - 0x1c800000u) >= (0x5d800000u - 0x1c800000u);
         dst[i] = v;
@@ -394,7 +433,14 @@ cudaError_t rb_lanes_launch_sum_slots(const float* d_partial, const uint32_t* d_
 cudaError_t rb_lanes_fifo_scatter(const float* d_staging, const rb_fifo_job* d_jobs, uint32_t n_jobs, float* d_fifo, uint64_t stride,
                                   uint32_t* d_flags, cudaStream_t st) {
     if (n_jobs == 0) return cudaSuccess;
-    k_fifo_scatter<<<n_jobs, 128, 0, st>>>(d_staging, d_jobs, d_fifo, stride, d_flags);
+    k_fifo_scatter<false><<<n_jobs, 128, 0, st>>>(d_staging, d_jobs, d_fifo, stride, d_flags, nullptr);
+    return cudaGetLastError();
+}
+
+cudaError_t rb_lanes_fifo_scatter_prog(const float* d_staging, const rb_fifo_prog_job* d_jobs, uint32_t n_jobs, const rb_prog_op* d_ops,
+                                       float* d_fifo, uint64_t stride, uint32_t* d_flags, cudaStream_t st) {
+    if (n_jobs == 0) return cudaSuccess;
+    k_fifo_scatter<true><<<n_jobs, 128, 0, st>>>(d_staging, d_jobs, d_fifo, stride, d_flags, d_ops);
     return cudaGetLastError();
 }
 

@@ -4,6 +4,7 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "rb_internal.h"
 #include "rb_lanes_core.h"
 
 // One stream of a batch that fits the lane kernel's shape (C = 1 or 2 interleaved channels, the mixer has the same C):
@@ -96,6 +97,26 @@ struct rb_fifo_job {          // one row of one push, 24 bytes
 // flags[row] becomes non-zero (and stays so) when one of them lies outside the exact-reciprocal class.  One CTA per job.
 cudaError_t rb_lanes_fifo_scatter(const float* d_staging, const rb_fifo_job* d_jobs, uint32_t n_jobs, float* d_fifo, uint64_t stride,
                                   uint32_t* d_flags, cudaStream_t st);
+// ---- push programs: the closed-form adapters a source's chain begins with (rb_dsp.cuh), applied as the PCM is pushed ----
+// kind: RB_N_AMPLIFY, RB_N_RAMP, RB_N_TAKE or RB_N_DISTORT (rb_internal.h), with the parameters the batch planner gives them.
+struct rb_prog_op {
+    uint32_t kind, pad_;
+    union {
+        float amp;
+        rb_dist_params dist;
+        rb_ramp_params ramp;
+        rb_take_params take;
+    } p;
+};
+struct rb_fifo_prog_job {     // a job of a session with push programs, 40 bytes
+    rb_fifo_job j;
+    uint64_t base;            // frames of the source that went through its program before this push
+    uint32_t op0, n_ops;      // the source's program: ops[op0, op0 + n_ops) (n_ops = 0: none)
+};
+// The same scatter with every sample n = (base + f) * src_ch + ch0 + c of the source first run through the job's program, in
+// chain order, and classified after it.
+cudaError_t rb_lanes_fifo_scatter_prog(const float* d_staging, const rb_fifo_prog_job* d_jobs, uint32_t n_jobs, const rb_prog_op* d_ops,
+                                       float* d_fifo, uint64_t stride, uint32_t* d_flags, cudaStream_t st);
 // FIFO compaction into the other arena: dst[r][0, keep[r]) = src[r][drop[r], drop[r] + keep[r]).
 cudaError_t rb_lanes_fifo_compact(const float* d_src, float* d_dst, uint64_t stride, const uint32_t* d_drop, const uint32_t* d_keep,
                                   uint32_t n_streams, cudaStream_t st);

@@ -694,7 +694,9 @@ class Session:
     """Streaming mixer: sources whose PCM arrives block by block (decoders, live input), the mixer output pulled block by
     block -- the block form of MixerSource::next (src/mixer.rs:120-136).  Any split into pushes and renders gives the
     bytes of the whole-stream Batch render with RB_FUSED_LANES.  `sources` describe the chains
-    (UniformSourceIterator(src, 1, rate)[.low_pass / .high_pass][.amplify]); their pcm is ignored."""
+    (UniformSourceIterator(src, 1, rate)[.low_pass / .high_pass][.amplify]); their pcm is ignored.  A chain may begin with a push
+    program -- fade_in / fade_out / linear_gain_ramp / take_duration / distortion, with amplify and speed among them -- applied as
+    the PCM is pushed; a take ends its source, and later pushes are dropped (include/rodio_b200.h has the takes served)."""
 
     def __init__(self, sources: Sequence[Source], mixer_rate: int, fifo_frames: int = 8192, max_block_frames: int = 4096,
                  mix_starts: Optional[Sequence[int]] = None, ctx: Optional[Context] = None, mixer_channels: Optional[int] = None,
@@ -746,6 +748,11 @@ class Session:
         n = (C.c_uint64 * len(blocks))(*[b.size // ch for b, ch in zip(blocks, self.src_channels)])
         eos = (C.c_uint8 * len(blocks))(*[int(bool(e)) for e in end_of_stream]) if end_of_stream is not None else None
         check(lib().rb_session_push_packed(self._h, flat.ctypes.data_as(C.c_void_p), n, eos), "rb_session_push_packed")
+
+    def push_silence(self, stream: int, n_frames: int):
+        """Player::pause for `n_frames` frames: whole frames of 0.0 behind the source's push program, which is not pulled meanwhile
+        (its fades and takes stand still), as Pausable does (src/source/pausable.rs:85-97).  Refused for a filter in front."""
+        check(lib().rb_session_push_silence(self._h, stream, int(n_frames)), "rb_session_push_silence")
 
     def start(self, stream: int):
         """Mixer::add for a source created with mix_start = capi.RB_SESSION_HELD: joins at the frame rendered next."""
@@ -921,8 +928,8 @@ class Player:
     mixer's format on its own); `pause()` / `play()` at known positions are the `pauses` of `append` (Pausable sits between the
     speed and the volume, player.rs:122-128: the source and its filters are not pulled while paused, whole frames of zeros go
     out -- RB_FX_PAUSE).  This class renders offline; the controls WHILE playing live on a `Session`: `follow` (append),
-    `set_volume` (the Amplify in front of the mixer's conversion, per pulled frame), pausing = pushing zero frames, stop / skip =
-    end_of_stream (INTEGRATION.md, examples/live_player.c).  Seeking is a control-plane feature of the decoders and out of
+    `set_volume` (the Amplify in front of the mixer's conversion, per pulled frame), pausing = `push_silence` (frames of zeros
+    behind the source's fades and takes, which stand still), stop / skip = end_of_stream (INTEGRATION.md, examples/live_player.c).  Seeking is a control-plane feature of the decoders and out of
     scope (SURVEY.md §2)."""
 
     def __init__(self, mixer: "Mixer"):
