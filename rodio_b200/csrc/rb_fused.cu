@@ -571,7 +571,10 @@ __device__ __forceinline__ void cta_bar() { asm volatile("bar.sync 0;" ::: "memo
 #ifdef RB_HOT_TIMING
 // Instrumented build (tools/hot_timing.py): cycles each warp spends working / waiting at the tile barrier.
 __device__ unsigned long long g_hot_timing[32][4];   // work, barrier, window wait, -
-__device__ int g_hot_skip;   // bit 0: no stage A, bit 1: no recurrence, bit 2: no stage C, bit 3: no second rows (results are wrong)
+// bit 0: no stage A, bit 1: no recurrence, bit 2: no stage C, bit 3: no second rows, bit 4: conflict-free window addresses, bit 5:
+// no range check, bit 6: no stage-A t stores (results are wrong).  In constant memory: read-only to the kernel, so the compiler
+// may keep it in a uniform register across the shared-memory stores of stage A.
+__constant__ int g_hot_skip;
 #define HOT_SKIP(bit) (g_hot_skip_v & (bit))
 #define HOT_TIMING_DECL long long tw_ = 0, tb_ = 0, tm_ = 0, tt0_ = clock64(), tt1_ = 0; const int g_hot_skip_v = g_hot_skip;
 #define HOT_MBAR_WAIT(bar_, ph_) do { const long long m0_ = clock64(); mbar_wait(bar_, ph_); tm_ += clock64() - m0_; } while (0)
@@ -748,9 +751,22 @@ __device__ __forceinline__ void hot_ff_store(float b0, float b1, float b2, const
 #pragma unroll
         for (int u = 0; u < P; u++) tv[u] = xv[u];
     }
-    float4* o = reinterpret_cast<float4*>(row + P * lane);
+#ifdef RB_HOT_TIMING
+    if (g_hot_skip & 64) {   // ablation: no t stores (a test that almost never passes keeps the feed-forward live)
+        uint32_t h = 0;
 #pragma unroll
-    for (int u = 0; u < P; u += 4) o[u / 4] = make_float4(tv[u], tv[u + 1], tv[u + 2], tv[u + 3]);
+        for (int u = 0; u < P; u++) h ^= __float_as_uint(tv[u]);
+        if (h != 0x7fbadbadu) return;
+    }
+#endif
+    // Lanes l and l + 4 cover the same banks with 16-byte stores at a 32-byte lane stride.  In the mono kernel the lanes with
+    // (l >> 2) & 1 write their second 16 bytes first, so that each 8-lane phase of an STS.128 covers all 32 banks once.
+    static_assert(P == 8, "two 16-byte stores per lane");
+    const float4 v0 = make_float4(tv[0], tv[1], tv[2], tv[3]), v1 = make_float4(tv[4], tv[5], tv[6], tv[7]);
+    const bool sw = C == 1 && ((lane >> 2) & 1u);
+    float4* o = reinterpret_cast<float4*>(row + P * lane);
+    o[sw ? 1 : 0] = sw ? v1 : v0;
+    o[sw ? 0 : 1] = sw ? v0 : v1;
 }
 
 template <bool NOGAIN, int C, bool HASB>
@@ -782,17 +798,42 @@ __device__ __forceinline__ void hot_stage_a(const FusedRow& r, const HotTile& ht
             float nf = __uint2float_rn(num);
             bool bad = false;
             float xv[P];
-#pragma unroll
-            for (int f = 0; f < F; f++) {
+            if (step_w == 0) {
+                // from < to: only the right tap is loaded, the left one is the previous frame's right (index moved) or left tap
+                // (hot_stage_a_pair)
                 float x0[C], x1[C];
 #pragma unroll
                 for (int c = 0; c < C; c++) x0[c] = w[c], x1[c] = w[C + c];
-                const float nfc = nf;
-                nf = add(nf, r1f);
-                w += step_w;
-                if (nf >= den_f) nf = sub(nf, den_f), w += C;
 #pragma unroll
-                for (int c = 0; c < C; c++) xv[f * C + c] = hot_lerp<NOGAIN>(x0[c], x1[c], nfc, den_f, rcp_den, pre, n_pre, mid, n_mid, bad);
+                for (int f = 0; f < F; f++) {
+                    const float nfc = nf;
+                    nf = add(nf, r1f);
+                    const bool carry = nf >= den_f;
+                    if (carry) nf = sub(nf, den_f), w += C;
+#pragma unroll
+                    for (int c = 0; c < C; c++) xv[f * C + c] = hot_lerp<NOGAIN>(x0[c], x1[c], nfc, den_f, rcp_den, pre, n_pre, mid, n_mid, bad);
+                    if (f + 1 < F) {
+#pragma unroll
+                        for (int c = 0; c < C; c++) {
+                            const float x2 = w[C + c];
+                            x0[c] = carry ? x1[c] : x0[c];
+                            x1[c] = x2;
+                        }
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int f = 0; f < F; f++) {
+                    float x0[C], x1[C];
+#pragma unroll
+                    for (int c = 0; c < C; c++) x0[c] = w[c], x1[c] = w[C + c];
+                    const float nfc = nf;
+                    nf = add(nf, r1f);
+                    w += step_w;
+                    if (nf >= den_f) nf = sub(nf, den_f), w += C;
+#pragma unroll
+                    for (int c = 0; c < C; c++) xv[f * C + c] = hot_lerp<NOGAIN>(x0[c], x1[c], nfc, den_f, rcp_den, pre, n_pre, mid, n_mid, bad);
+                }
             }
             if (!__any_sync(0xffffffffu, bad)) {
                 hot_ff_store<C, HASB>(b0, b1, b2, xv, xtail, lane, row);
@@ -866,20 +907,43 @@ __device__ __forceinline__ bool hot_stage_a_pair(const FusedRow& ra, const Fused
     if (num >= to) num -= to, di += 1;
     const float* w = win_a + ha.woff + di;
     const int db = (int)((win_b + hb.woff) - (win_a + ha.woff));   // row b's taps relative to row a's (warp-uniform)
+#ifdef RB_HOT_TIMING
+    if (g_hot_skip & 16) w = win_a + lane;        // ablation: conflict-free (wrong) window addresses
+#endif
     const uint32_t step_w = ra.q32;
     const float r1f = __uint2float_rn(ra.r32);
     float nf = __uint2float_rn(num);
     bool bad = false;
     float xa[P], xb[P];
+    if (step_w == 0) {
+        // from < to (q32 == 0): the window index moves by 0 or 1 word per frame.  When it moves, the next frame's left tap is this
+        // frame's right tap; when it stays, both taps stay.  So only the right tap is loaded: one LDS per frame and row.
+        float a0 = w[0], a1 = w[1], b0 = w[db], b1 = w[db + 1];
 #pragma unroll
-    for (int f = 0; f < P; f++) {
-        const float a0 = w[0], a1 = w[1], b0 = w[db], b1 = w[db + 1];
-        const float nfc = nf;
-        nf = add(nf, r1f);
-        w += step_w;
-        if (nf >= den_f) nf = sub(nf, den_f), w += 1;
-        xa[f] = hot_lerp<NOGAIN>(a0, a1, nfc, den_f, rcp_den, ra.pre, n_pre, ra.mid, n_mid, bad);
-        xb[f] = hot_lerp<NOGAIN>(b0, b1, nfc, den_f, rcp_den, rb.pre, n_pre, rb.mid, n_mid, bad);
+        for (int f = 0; f < P; f++) {
+            const float nfc = nf;
+            nf = add(nf, r1f);
+            const bool carry = nf >= den_f;
+            if (carry) nf = sub(nf, den_f), w += 1;
+            xa[f] = hot_lerp<NOGAIN>(a0, a1, nfc, den_f, rcp_den, ra.pre, n_pre, ra.mid, n_mid, bad);
+            xb[f] = hot_lerp<NOGAIN>(b0, b1, nfc, den_f, rcp_den, rb.pre, n_pre, rb.mid, n_mid, bad);
+            if (f + 1 < P) {
+                const float a2 = w[1], b2 = w[db + 1];
+                a0 = carry ? a1 : a0, b0 = carry ? b1 : b0;
+                a1 = a2, b1 = b2;
+            }
+        }
+    } else {
+#pragma unroll
+        for (int f = 0; f < P; f++) {
+            const float a0 = w[0], a1 = w[1], b0 = w[db], b1 = w[db + 1];
+            const float nfc = nf;
+            nf = add(nf, r1f);
+            w += step_w;
+            if (nf >= den_f) nf = sub(nf, den_f), w += 1;
+            xa[f] = hot_lerp<NOGAIN>(a0, a1, nfc, den_f, rcp_den, ra.pre, n_pre, ra.mid, n_mid, bad);
+            xb[f] = hot_lerp<NOGAIN>(b0, b1, nfc, den_f, rcp_den, rb.pre, n_pre, rb.mid, n_mid, bad);
+        }
     }
     if (__any_sync(0xffffffffu, bad)) return false;
     hot_ff_store<1, HASB>(ra.b0, ra.b1, ra.b2, xa, tail_a, lane, row_a);

@@ -1,10 +1,13 @@
 #!/usr/bin/env python
 """Where does a tile iteration of k_fused_hot go?  Builds an instrumented copy of the library
 (-DRB_HOT_TIMING: clock64 around each warp's work and its wait at the tile barrier), runs the bench
-workload once and prints, per warp, the share of cycles spent working vs waiting.  Diagnostic only."""
+workload once and prints, per warp, the share of cycles spent working vs waiting.  Diagnostic only.
+--ablate-smem: the full kernel, conflict-free window addresses (bit 16) and no stage-A t stores (bit 64), three
+renders each in turn, to bound what stage A's shared-memory traffic costs."""
 import ctypes as C
 import json
 import os
+import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -27,6 +30,9 @@ from rodio_b200 import dist as rbd  # noqa: E402
 def main():
     S = int(sys.argv[1]) if len(sys.argv) > 1 and sys.argv[1].isdigit() else 4096
     ch = 2 if "--stereo" in sys.argv else 1
+    q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True)
+    print("gpu:", q.stdout.strip() or q.stderr.strip())
     ctx = rb.default_context(0)
     dev = torch.device("cuda", 0)
     ext = torch.cuda.ExternalStream(ctx.cuda_stream, device=dev)
@@ -45,7 +51,10 @@ def main():
         skips = [0, 1, 2, 4, 8, 1 | 4 | 8, 2 | 4, 1 | 2 | 4] if "--skips" in sys.argv else [0]
         if "--ablate" in sys.argv:
             skips = [0, 1 | 4 | 8, 2 | 4, 2]
-        names = {1: "no stage A", 2: "no recurrence", 4: "no stage C", 8: "no second rows", 16: "conflict-free window reads", 32: "no range check"}
+        if "--ablate-smem" in sys.argv:
+            skips = [0, 16, 64] * 3
+        names = {1: "no stage A", 2: "no recurrence", 4: "no stage C", 8: "no second rows", 16: "conflict-free window reads", 32: "no range check",
+                 64: "no stage-A t stores"}
         for skip in skips:
             lib.rb_debug_hot_skip(skip)
             lib.rb_debug_hot_timing(buf, 1)
