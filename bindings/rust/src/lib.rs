@@ -294,6 +294,7 @@ impl Source for GpuMixerSource {
 // and hands the rendered mixer frames out one by one.  State (resampler position, pending frames, filter state) lives
 // in the session, so the block size is free -- 10 ms blocks for a cpal callback, whole seconds for offline renders.
 pub enum rb_session {}
+pub const RB_SESSION_RESTARTS: u32 = 1;
 #[repr(C)]
 pub struct rb_wav_info { pub sample_rate: u32, pub channels: u16, pub bits_per_sample: u16, pub format: u16, pub packed24: u16, pub pad_: u32,
                          pub data_offset: u64, pub data_bytes: u64, pub n_samples: u64 }
@@ -301,6 +302,12 @@ pub struct rb_wav_info { pub sample_rate: u32, pub channels: u16, pub bits_per_s
 extern "C" {
     fn rb_session_create(ctx: *mut rb_context, mixer_channels: u16, mixer_rate: u32, descs: *const rb_stream_desc, n: usize,
                          fifo_frames: u32, max_block_frames: u32, out: *mut *mut rb_session) -> i32;
+    /// `rb_session_create` with flags; `RB_SESSION_RESTARTS`: the conversion restarts every min(span_len, 32768) samples and
+    /// behind `take_duration`, as `UniformSourceIterator` does.
+    pub fn rb_session_create_ex(ctx: *mut rb_context, mixer_channels: u16, mixer_rate: u32, descs: *const rb_stream_desc, n: usize,
+                                fifo_frames: u32, max_block_frames: u32, flags: u32, out: *mut *mut rb_session) -> i32;
+    pub fn rb_session_source_runs(s: *mut rb_session, stream: usize, runs_started: *mut u64) -> i32;
+    pub fn rb_session_restart_launches(s: *mut rb_session, launches: *mut u64) -> i32;
     fn rb_session_destroy(s: *mut rb_session) -> i32;
     fn rb_session_push_packed(s: *mut rb_session, pcm: *const f32, n_frames: *const u64, end_of_stream: *const u8) -> i32;
     fn rb_session_push_silence(s: *mut rb_session, stream: usize, n_frames: u64) -> i32;

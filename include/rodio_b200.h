@@ -347,7 +347,8 @@ rb_status rb_batch_read_stream(rb_batch* b, size_t stream, float* out_host, uint
  * reaches it is cut there, later pushes are dropped with RB_OK.  Behind a take rodio's conversion restarts every 32768 samples
  * and never pulls the padding; sessions serve takes of one such run in whole frames, or sources at the mixer's rate whose
  * channels pass through or restart on a frame boundary (RB_ERR_UNSUPPORTED otherwise), and no filter behind a take that ends
- * inside a frame.  Sources of different shapes may share a session (classes of their own); desc.n_samples / span_len are ignored,
+ * inside a frame; rb_session_create_ex with RB_SESSION_RESTARTS follows those restarts.  Sources of different shapes may share a
+ * session (classes of their own); desc.n_samples / span_len are ignored (span_len: unless RB_SESSION_RESTARTS is given),
  * desc.mix_start is the mixer FRAME the source joins at.  Everything below counts frames; PCM is interleaved.
  * One caller per session; every call returns with the work done (the caller may reuse its buffers). */
 typedef struct rb_session rb_session;
@@ -357,7 +358,28 @@ typedef struct rb_session rb_session;
 /* fifo_frames: input frames a source can hold between renders (>= 64); max_block_frames: largest render. */
 rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels, uint32_t mixer_sample_rate, const rb_stream_desc* descs,
                             size_t n_streams, uint32_t fifo_frames, uint32_t max_block_frames, rb_session** out);
+/* rb_session_create with flags (0: the same call).  RB_SESSION_RESTARTS: the session restarts the mixer's conversion where rodio
+ * does.  UniformSourceIterator converts no source as one run: at every bootstrap it asks current_span_len(), caps the answer at
+ * 32768 samples and builds a fresh SampleRateConverter over that many samples, which interpolates inside itself only, emits its
+ * last frame raw and starts again at numerator 0 (src/source/uniform.rs:50-68, src/conversions/sample_rate.rs:58-71, :187-199).
+ * With the flag desc.span_len means what it means in batches: 0 = None, one run for the whole source; S > 0 = the source reports
+ * Some(S) at every bootstrap (a SamplesBuffer: its length; a decoder: its packet), so runs are min(S, 32768) samples until the
+ * input ends.  desc.n_samples stays ignored.  A resampled source whose push program holds a TAKE_DURATION restarts every
+ * min(samples left in the take, S, 32768) samples, the frames of rb_session_push_silence counted against the run as rodio's Take
+ * counts Pausable's zeros: such takes may be longer than one run and may be paused.  Filter state and gains carry across a
+ * restart, for any split into pushes and renders.  A source at the mixer's rate keeps no conversion state: its restarts change
+ * nothing and are not tracked.  RB_ERR_UNSUPPORTED: a schedule whose runs are not whole frames of the source (span_len not a
+ * multiple of its channel count; 3, 5, 6, 7 ... channels under the 32768 cap; a resampled take that ends inside a frame) and runs
+ * shorter than two frames.  Such a session writes state blob version 8 when some source has a schedule. */
+#define RB_SESSION_RESTARTS 1u
+rb_status rb_session_create_ex(rb_context* ctx, uint16_t mixer_channels, uint32_t mixer_sample_rate, const rb_stream_desc* descs,
+                               size_t n_streams, uint32_t fifo_frames, uint32_t max_block_frames, uint32_t flags, rb_session** out);
 rb_status rb_session_destroy(rb_session* s);
+/* Converter runs of source `stream` that have produced an output so far (1 once a source without a schedule plays; sources at
+ * the mixer's rate: see RB_SESSION_RESTARTS), and the launches of the lane kernel's RESTART variants so far: a block in which no
+ * source restarts makes none. */
+rb_status rb_session_source_runs(rb_session* s, size_t stream, uint64_t* runs_started);
+rb_status rb_session_restart_launches(rb_session* s, uint64_t* launches);
 /* mixer_source.amplify(a).limit(settings).amplify(b) on the session's output: see rb_batch_set_master. */
 rb_status rb_session_set_master(rb_session* s, const rb_effect* effects, uint32_t n_effects);
 /* n_frames more frames of source `stream` have arrived; end_of_stream != 0: the source's Iterator::next would return
@@ -409,7 +431,8 @@ rb_status rb_session_render(rb_session* s, float* out_host, uint64_t max_frames,
  * context, continues bit-identically.  buf == NULL: only *size is returned.  One record per slot row; a session whose every
  * source is one row carrying all of its channels (mono and stereo mixers, mono sources in any mixer) writes version 5, any
  * other layout version 6 with a layout record per row; a session with push programs writes version 7, which adds the program
- * frames each source has consumed and the programs.  A blob of another shape, layout, master chain or program: RB_ERR_INVALID_ARGUMENT. */
+ * frames each source has consumed and the programs; a session with restart schedules writes version 8, which adds the converter
+ * run of each source.  A blob of another shape, schedule, layout, master chain or program: RB_ERR_INVALID_ARGUMENT. */
 rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap, uint64_t* size);
 rb_status rb_session_set_state(rb_session* s, const void* buf, uint64_t size);
 

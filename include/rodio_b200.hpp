@@ -365,19 +365,28 @@ inline std::pair<Mixer, MixerSource> mixer(uint16_t channels, uint32_t sample_ra
 class LiveMixer {
   public:
     // mixer::mixer(channels, sample_rate) whose inputs arrive later: chains[i] ends in .uniform(channels, sample_rate)...
+    // restarts: RB_SESSION_RESTARTS -- the mixer's conversion restarts where rodio's does, every min(span_len, 32768) samples of a
+    // chain whose source reports a span, and behind take_duration.
     LiveMixer(const std::vector<Source>& chains, uint16_t channels, uint32_t sample_rate, uint32_t fifo_frames = 8192,
-              uint32_t block_frames = 1024)
+              uint32_t block_frames = 1024, bool restarts = false)
         : channels_(channels), rate_(sample_rate), block_frames_(block_frames) {
         std::vector<rb_stream_desc> descs;
         for (const Source& c : chains) descs.push_back(c.desc(0)), src_channels_.push_back(descs.back().channels);
-        check(rb_session_create(Context::get(), channels, sample_rate, descs.data(), descs.size(), fifo_frames, block_frames, &h_),
-              "rb_session_create");
+        check(rb_session_create_ex(Context::get(), channels, sample_rate, descs.data(), descs.size(), fifo_frames, block_frames,
+                                   restarts ? RB_SESSION_RESTARTS : 0u, &h_),
+              "rb_session_create_ex");
     }
     LiveMixer(const LiveMixer&) = delete;
     LiveMixer& operator=(const LiveMixer&) = delete;
     ~LiveMixer() { rb_session_destroy(h_); }
     uint16_t channels() const { return channels_; }
     uint32_t sample_rate() const { return rate_; }
+    // converter runs of source `i` that have produced an output so far (rb_session_source_runs)
+    uint64_t source_runs(size_t i) const {
+        uint64_t n = 0;
+        check(rb_session_source_runs(h_, i, &n), "rb_session_source_runs");
+        return n;
+    }
     // more interleaved samples of source `i`; end_of_stream: its Iterator::next would return None after them
     void push(size_t i, const std::vector<Sample>& pcm, bool end_of_stream = false) {
         check(rb_session_push(h_, i, pcm.data(), pcm.size() / src_channels_.at(i), end_of_stream ? 1 : 0), "rb_session_push");

@@ -39,6 +39,7 @@ RB_KEEP_STREAM_OUTPUTS = 1 << 3
 RB_FUSED_LANES = 1 << 4
 RB_FUSED_DUO = 1 << 5
 RB_SESSION_HELD = (1 << 64) - 1
+RB_SESSION_RESTARTS = 1
 
 
 class rb_effect(C.Structure):
@@ -98,6 +99,10 @@ SYMBOLS = {
     "rb_comm_transport": (C.c_int32, [C.c_void_p, C.c_char_p, C.c_uint64]),
     "rb_batch_render_mix_allreduce": (C.c_int32, [C.POINTER(C.c_void_p), C.c_int, C.c_void_p]),
     "rb_session_create": (C.c_int32, [C.c_void_p, C.c_uint16, C.c_uint32, C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]),
+    "rb_session_create_ex": (C.c_int32, [C.c_void_p, C.c_uint16, C.c_uint32, C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
+                                         C.POINTER(C.c_void_p)]),
+    "rb_session_source_runs": (C.c_int32, [C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64)]),
+    "rb_session_restart_launches": (C.c_int32, [C.c_void_p, C.POINTER(C.c_uint64)]),
     "rb_session_destroy": (C.c_int32, [C.c_void_p]),
     "rb_session_push": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint64, C.c_int]),
     "rb_session_push_packed": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

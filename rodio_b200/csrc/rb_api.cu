@@ -1816,6 +1816,10 @@ struct rb_session {
     std::vector<uint8_t> no_silence;           // a take in front of a resampling conversion: rb_session_push_silence refused
     rb_prog_op* d_prog = nullptr;
     rb_fifo_prog_job *d_pjobs = nullptr, *h_pjobs = nullptr;
+    // restart schedules (RB_SESSION_RESTARTS, rb_session_plan.h): some source has one; the cuts of a block, per row
+    bool has_sched = false;
+    lanes::Cut *d_cuts = nullptr, *h_cuts = nullptr;
+    uint64_t restart_launches = 0;             // launches of the lane kernel's RESTART twins so far
 #if defined(RB_SIMT_EMULATE)
     std::vector<uint64_t> emu_fast_tiles;      // CPU build: fast tiles the emulator ran per class (rb_session_emu_fast_tiles)
 #endif
@@ -1829,13 +1833,21 @@ extern "C" rb_status rb_session_destroy(rb_session* s) {
     cudaFreeHost(s->h_rows), cudaFreeHost(s->h_u32), cudaFreeHost(s->h_jobs), cudaFreeHost(s->h_out);
     cudaFree(s->d_master[0]), cudaFree(s->d_master[1]), cudaFree(s->d_master_runs), cudaFreeHost(s->h_master_runs);
     cudaFree(s->d_prog), cudaFree(s->d_pjobs), cudaFreeHost(s->h_pjobs);
+    cudaFree(s->d_cuts), cudaFreeHost(s->h_cuts);
     delete s;
     return RB_OK;
 }
 
 extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels, uint32_t mixer_rate, const rb_stream_desc* descs,
                                        size_t n_streams, uint32_t fifo_frames, uint32_t max_block_frames, rb_session** out) {
+    return rb_session_create_ex(ctx, mixer_channels, mixer_rate, descs, n_streams, fifo_frames, max_block_frames, 0, out);
+}
+
+extern "C" rb_status rb_session_create_ex(rb_context* ctx, uint16_t mixer_channels, uint32_t mixer_rate, const rb_stream_desc* descs,
+                                          size_t n_streams, uint32_t fifo_frames, uint32_t max_block_frames, uint32_t flags, rb_session** out) {
     if (!ctx || !out || !descs) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
+    if (flags & ~(uint32_t)RB_SESSION_RESTARTS) return fail(RB_ERR_INVALID_ARGUMENT, "unknown session flags");
+    const bool restarts = (flags & RB_SESSION_RESTARTS) != 0;
     if (mixer_rate == 0 || mixer_channels == 0 || n_streams == 0 || n_streams > 0x7FFFFFFFull)
         return fail(RB_ERR_INVALID_ARGUMENT, "zero mixer rate / channels or no streams");
     if (mixer_channels > RB_MAX_CHANNELS) return fail(RB_ERR_UNSUPPORTED, "mixer: more than 12 channels");
@@ -1853,6 +1865,7 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
     std::vector<std::vector<rb_prog_op>> progs(n);
     std::vector<uint64_t> take_n(n, ~0ull);   // samples the source's takes let through
     std::vector<uint8_t> no_silence(n, 0);
+    std::vector<uint64_t> run_cap(n, 0);      // RB_SESSION_RESTARTS: frames per converter run (0: the source is one run)
     for (size_t i = 0; i < n; i++) {
         const rb_stream_desc& d = descs[i];
         const std::string where = "stream " + std::to_string(i) + ": ";
@@ -1927,6 +1940,19 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
         from[i] = rate / g, to[i] = mixer_rate / g;
         const bool filtered = k0 + 1 < d.n_effects && (d.effects[k0 + 1].kind == RB_FX_LOW_PASS || d.effects[k0 + 1].kind == RB_FX_HIGH_PASS);
         if (front && filtered) return fail(RB_ERR_UNSUPPORTED, where + "one filter per source: in front of the conversion or behind it");
+        // With RB_SESSION_RESTARTS the mixer's conversion is restarted where rodio restarts it: every min(span_len, 32768) samples,
+        // behind a take every min(samples left in the take, 32768).  Served when every run is whole frames of the source.
+        const bool cap_whole = RB_UNIFORM_SPAN_CAP % d.channels == 0;
+        bool take_runs = false;   // a resampled take that the schedule follows
+        if (restarts) {
+            if (d.span_len % d.channels || (d.span_len > RB_UNIFORM_SPAN_CAP && !cap_whole))
+                return fail(RB_ERR_UNSUPPORTED, where + "restarts: span_len (capped at 32768 samples) must be whole frames of the source");
+            take_runs = from[i] != to[i] && take_n[i] != ~0ull && take_n[i] % d.channels == 0 && (take_n[i] <= RB_UNIFORM_SPAN_CAP || cap_whole);
+            if (from[i] != to[i] && (d.span_len || take_runs)) {
+                run_cap[i] = d.span_len ? std::min(d.span_len, RB_UNIFORM_SPAN_CAP) / d.channels : cap_whole ? RB_UNIFORM_SPAN_CAP / d.channels : take_n[i] / d.channels;
+                if (run_cap[i] < 2) return fail(RB_ERR_UNSUPPORTED, where + "restarts: converter runs shorter than two frames");
+            }
+        }
         if (take_n[i] != ~0ull) {
             // Behind a take the mixer's conversion re-bootstraps every min(samples left, 32768) samples (src/source/uniform.rs:50-68,
             // take.rs:180-196) and never pulls the padding of the take's last frame.  A session converts the source as one run, with
@@ -1936,13 +1962,13 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
             const bool whole = take_n[i] % C_in == 0;
             const bool one_run = whole && take_n[i] <= RB_UNIFORM_SPAN_CAP;
             const bool stateless = from[i] == to[i] && (take_n[i] <= RB_UNIFORM_SPAN_CAP || C_in == 1 || C_in == mixer_channels || RB_UNIFORM_SPAN_CAP % C_in == 0);
-            if (!one_run && !stateless)
+            if (!one_run && !stateless && !take_runs)
                 return fail(RB_ERR_UNSUPPORTED, where + "take_duration: the mixer's conversion restarts every 32768 samples behind a take; "
                                                         "sessions serve longer takes (or takes that end inside a frame) at the mixer's rate only");
             if (!whole && (front || filtered))
                 return fail(RB_ERR_UNSUPPORTED, where + "a take that ends inside a frame pads it with 0.0, which a filter would see (rodio never pulls it)");
             // Pausable passes the take's span on: the conversion then counts the pause's zeros against the take and restarts early
-            if (from[i] != to[i]) no_silence[i] = 1;
+            if (from[i] != to[i] && !take_runs) no_silence[i] = 1;
         }
         // filtered / unfiltered sources, sources with / without a gain in front and sources whose filter sits in front are
         // classes of their own (a filter in front always applies the gains around it: no class of its own for those)
@@ -2005,6 +2031,7 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
                 return fail(RB_ERR_UNSUPPORTED, where + "the conversion pads channels with 0.0 and the filter or gain behind it is not finite (rodio gives NaN there)");
         }
         s->st[r].mix_start = d.mix_start, s->st[r].from = from[i], s->st[r].to = to[i];
+        s->st[r].run_cap = run_cap[i], s->has_sched = s->has_sched || run_cap[i] != 0;
         if (d.mix_start == RB_SESSION_HELD) s->st[r].held = true, s->st[r].mix_start = 0;   // Mixer::add comes later (rb_session_start)
         s->src_ch[r] = (uint8_t)d.channels;
         s->max_src_ch = std::max<uint32_t>(s->max_src_ch, d.channels);
@@ -2081,6 +2108,10 @@ extern "C" rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels,
     RB_CUDA(cudaMallocHost(&s->h_u32, 2 * nr * sizeof(uint32_t)));
     RB_CUDA(cudaMallocHost(&s->h_jobs, nr * sizeof(rb_fifo_job)));
     RB_CUDA(cudaMallocHost(&s->h_out, pstride * sizeof(float)));
+    if (s->has_sched) {
+        RB_CUDA(cudaMalloc(&s->d_cuts, nr * sizeof(lanes::Cut)));
+        RB_CUDA(cudaMallocHost(&s->h_cuts, nr * sizeof(lanes::Cut)));
+    }
     RB_CUDA(cudaMemsetAsync(s->d_fifo[0], 0, arena, ctx->stream));
     RB_CUDA(cudaMemsetAsync(s->d_fifo[1], 0, arena, ctx->stream));
     RB_CUDA(cudaMemsetAsync(s->d_state, 0, nr * 8 * sizeof(float), ctx->stream));
@@ -2131,6 +2162,7 @@ static uint64_t session_take_room(const rb_session* s, size_t r, uint64_t n) {
 }
 // After `frames` frames went into source r: its program index advances; the take's last frame ends the source.
 static void session_pushed(rb_session* s, size_t r, uint64_t frames) {
+    session::schedule_push(s->st[r], frames, s->prog_end[r] == ~0ull ? ~0ull : s->prog_end[r] - std::min(s->prog_end[r], s->prog_pos[r]), true);
     s->st[r].pushed += frames;
     s->prog_pos[r] += frames;
     if (session_take_ended(s, r)) s->st[r].eof = true;
@@ -2177,6 +2209,7 @@ extern "C" rb_status rb_session_push_silence(rb_session* s, size_t stream, uint6
         RB_CUDA(cudaMemsetAsync(s->d_fifo[s->cur] + q * s->stride + st.fill() * ci, 0, n_frames * ci * sizeof(float), stq));
     }
     RB_CUDA(cudaStreamSynchronize(stq));
+    session::schedule_push(st, n_frames, s->prog_end[r] == ~0ull ? ~0ull : s->prog_end[r] - std::min(s->prog_end[r], s->prog_pos[r]), false);
     st.pushed += n_frames;   // the program's index stands still
     return RB_OK;
 }
@@ -2307,6 +2340,8 @@ extern "C" rb_status rb_session_available(rb_session* s, uint64_t* frames, int* 
     return RB_OK;
 }
 
+static rb_status session_render_block(rb_session* s, float* out_host, uint64_t n);
+
 extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t max_frames, uint64_t* written, int* ended) {
     if (!s || !written) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
     *written = 0;
@@ -2316,6 +2351,29 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
     if (ended) *ended = e ? 1 : 0;
     if (n == 0) return RB_OK;
     if (!out_host) return fail(RB_ERR_INVALID_ARGUMENT, "out_host is NULL");
+    // The lane kernel walks one restart per row and launch: a block in which some source restarts twice (spans of a few frames)
+    // is rendered as sub-blocks that end where such a source's second run does.
+    while (*written < n) {
+        uint64_t k = n - *written;
+        if (s->has_sched)
+            for (session::Stream& st : s->st) {
+                session::settle(st);
+                if (!st.held && !session::finished(st)) k = std::min(k, session::one_cut_limit(st) - std::min(session::one_cut_limit(st), s->T));
+            }
+        rb_status rc = session_render_block(s, out_host + *written * s->channels, k);
+        if (rc != RB_OK) return rc;
+        *written += k;
+    }
+    if (ended) {
+        bool e2 = false;
+        session::renderable(s->st, s->T, 1, &e2);
+        *ended = e2 ? 1 : 0;
+    }
+    return RB_OK;
+}
+
+// One launch per class over the frames [T, T + n), which every source can supply and in which none restarts twice.
+static rb_status session_render_block(rb_session* s, float* out_host, uint64_t n) {
     RB_CUDA(cudaSetDevice(s->ctx->device));
     cudaStream_t stq = s->ctx->stream;
     const size_t ns = s->st.size(), nr = s->rows.size();
@@ -2328,13 +2386,19 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
         if (!s->st[r].front && !(lanes::pre_gain_keeps_class(s->pre[r]) && lanes::pre_gain_keeps_class(s->vol_a[r]) && lanes::pre_gain_keeps_class(s->vol_b[r])))
             quiet[r] = 1;   // its class runs the guarded tile in this block (or, DOWN, slow tiles)
     }
+    bool any_cut = false;
     for (size_t q = 0; q < nr; q++) {   // every row of a source renders the source's part: the rows stay in lock step
         const size_t r = s->rows[q].src;
         const session::Part& p = parts[r];
         lanes::Row& row = s->h_rows[q];
         memset(&row, 0, sizeof(row));
-        row.in = fifo + q * s->stride, row.L = s->st[r].fill(), row.out_len = p.out_len, row.mix_start = p.mix_start;
-        row.n_int = p.n_int, row.o0 = p.o0, row.i0 = s->st[r].i0, row.state = s->d_state + 8 * q;
+        // positions are relative to the converter run of the block's first output (without a schedule: the whole stream)
+        row.in = fifo + q * s->stride, row.L = p.out_len ? p.run_end - s->st[r].i0 : s->st[r].fill(), row.out_len = p.out_len, row.mix_start = p.mix_start;
+        row.n_int = p.n_int, row.o0 = p.o0, row.i0 = s->st[r].i0 - p.run_i, row.state = s->d_state + 8 * q;
+        if (s->has_sched) {
+            s->h_cuts[q] = lanes::Cut{p.cut_m, p.cut_n_int, s->st[r].i0 - p.cut_i, p.cut_end - s->st[r].i0};
+            any_cut = any_cut || p.cut_m < p.out_len;
+        }
         const float* co = &s->coef[5 * r];
         row.b0 = co[0], row.b1 = co[1], row.b2 = co[2], row.a1 = co[3], row.a2 = co[4], row.ffk = s->ffk[r];
         row.post = s->post[r], row.pre = s->pre[r], row.mid = s->mid[r];
@@ -2342,6 +2406,7 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
         row.f0 = s->st[r].fpos - s->st[r].i0, row.ga = s->vol_a[r], row.gb = s->vol_b[r];
     }
     RB_CUDA(cudaMemcpyAsync(s->d_rows, s->h_rows, nr * sizeof(lanes::Row), cudaMemcpyHostToDevice, stq));
+    if (any_cut) RB_CUDA(cudaMemcpyAsync(s->d_cuts, s->h_cuts, nr * sizeof(lanes::Cut), cudaMemcpyHostToDevice, stq));
     const uint64_t pstride = lanes::round_up_tile((uint64_t)s->max_block * C);
     // rows of the partial buffer are only written inside each warp's span: clear what this block may read
     RB_CUDA(cudaMemsetAsync(s->d_partial, 0, (size_t)s->n_groups * pstride * sizeof(float), stq));
@@ -2353,12 +2418,27 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
         lanes::fill_ratio(a, s0.from, s0.to, c.ch_out);
         a.mix_len = n, a.pstride = pstride;
         a.partial = s->d_partial + (size_t)g0 * pstride, a.zeros = s->d_zeros, a.unsafe = s->d_flags + c.first;
-        bool guard = false;
-        for (uint32_t q = c.first; q < c.first + c.count; q++) guard = guard || quiet[s->rows[q].src];
+        bool guard = false, cut = false;   // cut: some row of the class restarts in this block -- the class takes the RESTART twin
+        for (uint32_t q = c.first; q < c.first + c.count; q++) {
+            guard = guard || quiet[s->rows[q].src];
+            cut = cut || (any_cut && s->h_cuts[q].m < s->h_rows[q].out_len);
+        }
 #if defined(RB_SIMT_EMULATE)
         const uint64_t fast0 = simt::g_emu_count[0];
 #endif
-        RB_CUDA(rb_lanes_launch_kernel(a, c.ch_in, c.ch_out, c.has_biquad, c.ff2, s->has_post, c.has_pre, c.front, guard, stq));
+        if (cut) {
+            a.cuts = s->d_cuts + c.first;
+#if defined(RB_SIMT_EMULATE)
+            session_host::g_restart_readable.clear();
+            for (const auto& b : {std::pair<const void*, size_t>{fifo, nr * s->stride * sizeof(float)}, {s->d_rows, nr * sizeof(lanes::Row)}, {s->d_cuts, nr * sizeof(lanes::Cut)},
+                                  {s->d_state, nr * 8 * sizeof(float)}, {s->d_zeros, 256}, {s->d_flags, nr * sizeof(uint32_t)}})
+                session_host::g_restart_readable.push_back({(const char*)b.first, (const char*)b.first + b.second});
+#endif
+            RB_CUDA(rb_lanes_launch_restart(a, c.ch_in, c.ch_out, c.has_biquad, c.front, stq));
+            s->restart_launches++;
+        } else {
+            RB_CUDA(rb_lanes_launch_kernel(a, c.ch_in, c.ch_out, c.has_biquad, c.ff2, s->has_post, c.has_pre, c.front, guard, stq));
+        }
 #if defined(RB_SIMT_EMULATE)
         s->emu_fast_tiles[&c - s->classes.data()] += simt::g_emu_count[0] - fast0;
 #endif
@@ -2420,12 +2500,19 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
     if (s->has_master) s->master_k ^= 1;
     memcpy(out_host, s->h_out, n * C * sizeof(float));
     s->T += n;
-    *written = n;
-    if (ended) {
-        bool e2 = false;
-        session::renderable(s->st, s->T, 1, &e2);
-        *ended = e2 ? 1 : 0;
-    }
+    return RB_OK;
+}
+
+extern "C" rb_status rb_session_source_runs(rb_session* s, size_t stream, uint64_t* runs_started) {
+    if (!s || !runs_started) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
+    if (stream >= s->st.size()) return fail(RB_ERR_INVALID_ARGUMENT, "stream index out of range");
+    *runs_started = session::runs_started(s->st[s->pos[stream]]);
+    return RB_OK;
+}
+
+extern "C" rb_status rb_session_restart_launches(rb_session* s, uint64_t* launches) {
+    if (!s || !launches) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
+    *launches = s->restart_launches;
     return RB_OK;
 }
 
@@ -2473,8 +2560,20 @@ struct SessionBlobProg {
     uint64_t frames;                     // frames of the source that went through its program
     uint32_t op0, n_ops;
 };
+// Version 8 (a session some source of which has a restart schedule): version 6 or, with push programs, 7, then one run record per
+// source (source order), each followed by its n_ends run ends, then the FIFO contents.  A blob only restores a session with the
+// same schedules.
+struct SessionBlobRun {
+    uint64_t run_cap, run_i, run_o, sched_end, runs_done, n_ends;
+};
 constexpr uint32_t SESSION_MAGIC = 0x52425353u;   // "RBSS"
-uint32_t blob_version(const rb_session* s) { return s->has_prog ? 7u : s->plain ? 5u : 6u; }
+uint32_t blob_version(const rb_session* s) { return s->has_sched ? 8u : s->has_prog ? 7u : s->plain ? 5u : 6u; }
+uint64_t blob_run_bytes(const rb_session* s) {
+    uint64_t n = 0;
+    if (s->has_sched)
+        for (const session::Stream& st : s->st) n += sizeof(SessionBlobRun) + st.ends.size() * sizeof(uint64_t);
+    return n;
+}
 SessionBlobSlot blob_slot(const rb_session::Slot& sl) { return {sl.src, (uint32_t)sl.ch0 | (uint32_t)sl.w << 8 | (uint32_t)sl.ci << 16}; }
 // the fields a source's rows share
 bool same_source_fields(const SessionBlobStream& a, const SessionBlobStream& b) {
@@ -2489,7 +2588,7 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
     const size_t nr = s->rows.size(), ns = s->st.size();
     const uint64_t n_slots = blob_version(s) == 5u ? 0 : nr;
     const uint64_t prog_bytes = s->has_prog ? ns * sizeof(SessionBlobProg) + s->prog_ops.size() * sizeof(rb_prog_op) : 0;
-    uint64_t need = sizeof(SessionBlobHeader) + nr * sizeof(SessionBlobStream) + n_slots * sizeof(SessionBlobSlot) + prog_bytes;
+    uint64_t need = sizeof(SessionBlobHeader) + nr * sizeof(SessionBlobStream) + n_slots * sizeof(SessionBlobSlot) + prog_bytes + blob_run_bytes(s);
     const uint32_t C = s->channels;
     for (size_t q = 0; q < nr; q++) need += s->st[s->rows[q].src].fill() * s->rows[q].ci * sizeof(float);
     if (s->has_master) need += sizeof(SessionBlobMaster);
@@ -2520,6 +2619,12 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
         }
         memcpy(p, s->prog_ops.data(), s->prog_ops.size() * sizeof(rb_prog_op)), p += s->prog_ops.size() * sizeof(rb_prog_op);
     }
+    if (s->has_sched)
+        for (const session::Stream& st : s->st) {
+            const SessionBlobRun b{st.run_cap, st.run_i, st.run_o, st.sched_end, st.runs_done, st.ends.size()};
+            memcpy(p, &b, sizeof(b)), p += sizeof(b);
+            memcpy(p, st.ends.data(), st.ends.size() * sizeof(uint64_t)), p += st.ends.size() * sizeof(uint64_t);
+        }
     for (size_t q = 0; q < nr; q++) {
         const uint64_t fill = s->st[s->rows[q].src].fill() * s->rows[q].ci;   // floats
         if (fill) RB_CUDA(cudaMemcpyAsync(p, s->d_fifo[s->cur] + q * s->stride, fill * sizeof(float), cudaMemcpyDeviceToHost, s->ctx->stream));
@@ -2554,7 +2659,7 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
     if (size < sizeof(h)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
     memcpy(&h, p, sizeof(h)), p += sizeof(h);
     const uint32_t C = s->channels;
-    if (h.magic != SESSION_MAGIC || h.version < 5u || h.version > 7u) return fail(RB_ERR_INVALID_ARGUMENT, "not a session state blob");
+    if (h.magic != SESSION_MAGIC || h.version < 5u || h.version > 8u) return fail(RB_ERR_INVALID_ARGUMENT, "not a session state blob");
     if (h.version != blob_version(s) || h.n_streams != nr || h.has_biquad != (s->has_biquad ? 1u : 0u) || h.channels != C)
         return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session of another shape");
     uint64_t need = sizeof(h) + nr * sizeof(SessionBlobStream) + n_slots * sizeof(SessionBlobSlot) + prog_bytes;
@@ -2579,6 +2684,29 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
             return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session with other push programs");
         p += s->prog_ops.size() * sizeof(rb_prog_op);
     }
+    std::vector<session::Stream> runs(ns);   // the run records, checked against the source's record below
+    if (s->has_sched) {
+        const uint8_t* const end = (const uint8_t*)buf + size;
+        for (size_t r = 0; r < ns; r++) {
+            SessionBlobRun b;
+            if ((uint64_t)(end - p) < sizeof(b)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
+            memcpy(&b, p, sizeof(b)), p += sizeof(b);
+            if (b.run_cap != s->st[r].run_cap || (!b.run_cap && (b.n_ends || b.run_i || b.run_o)))
+                return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session with other restart schedules");
+            if (b.n_ends > (uint64_t)(end - p) / sizeof(uint64_t)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
+            session::Stream& st = runs[r];
+            st.run_cap = b.run_cap, st.run_i = b.run_i, st.run_o = b.run_o, st.sched_end = b.sched_end, st.runs_done = b.runs_done;
+            st.ends.resize(b.n_ends);
+            memcpy(st.ends.data(), p, b.n_ends * sizeof(uint64_t)), p += b.n_ends * sizeof(uint64_t);
+            need += sizeof(b) + b.n_ends * sizeof(uint64_t);
+            uint64_t at = b.run_i;   // runs follow one another, none shorter than a frame, the last one the pushes are filling
+            for (uint64_t e : st.ends) {
+                if (e <= at) return fail(RB_ERR_INVALID_ARGUMENT, "state blob: run record out of order");
+                at = e;
+            }
+            if (!st.ends.empty() && st.ends.back() != b.sched_end) return fail(RB_ERR_INVALID_ARGUMENT, "state blob: run record out of order");
+        }
+    }
     std::vector<uint8_t> first_row(nr, 0);
     for (const auto& rows : s->rows_of) first_row[rows[0]] = 1;
     for (size_t q = 0; q < nr; q++) {
@@ -2589,7 +2717,9 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
             return fail(RB_ERR_INVALID_ARGUMENT, "state blob: FIFO record out of range");
         if (b.follows < -1 || (b.follows >= 0 && ((size_t)b.follows >= nr || !first_row[(size_t)b.follows] || s->rows[(size_t)b.follows].src == r)))
             return fail(RB_ERR_INVALID_ARGUMENT, "state blob: queue record out of range");
-        if (b.out_done > session::out_total(b.pushed, b.from, b.to))
+        session::Stream chk = runs[r];   // with a schedule: the outputs its runs hold
+        chk.from = b.from, chk.to = b.to, chk.pushed = b.pushed, chk.eof = true;
+        if (b.out_done > session::out_end(chk) || b.out_done < chk.run_o || chk.run_i > b.pushed)
             return fail(RB_ERR_INVALID_ARGUMENT, "state blob: more outputs rendered than the pushed input holds");
         if (!same_source_fields(b, recs[s->rows_of[r][0]]))
             return fail(RB_ERR_INVALID_ARGUMENT, "state blob: the rows of one source disagree");
@@ -2613,6 +2743,7 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
         session::Stream& st = s->st[r];
         st.mix_start = b.mix_start, st.pushed = b.pushed, st.out_done = b.out_done, st.i0 = b.i0, st.eof = b.eof != 0, st.fpos = b.i0 + b.filter_ahead, s->vol_a[r] = b.vol_a, s->vol_b[r] = b.vol_b;
         st.held = b.held != 0, st.follows = b.follows < 0 ? -1 : (int64_t)s->rows[(size_t)b.follows].src;
+        st.run_i = runs[r].run_i, st.run_o = runs[r].run_o, st.sched_end = runs[r].sched_end, st.runs_done = runs[r].runs_done, st.ends = runs[r].ends;
         (st.front ? s->mid[r] : s->pre[r]) = b.vol;
         if (b.post != s->post[r]) s->post[r] = b.post, s->has_post = true;
     }

@@ -22,13 +22,13 @@ constexpr int lanes_rs() { return lanes::Geo<C, DOWN ? lanes::NSLOT_DOWN : RB_LA
 template <int C, bool DOWN>
 constexpr size_t lanes_smem_bytes() { return (size_t)LANES_WARPS * 32 * lanes_rs<C, DOWN>() * sizeof(float); }   // 21.0 KB
 
-template <int CI, int CO, bool HASB, bool FF2, int NPOST, bool PASS, bool PRE, bool FRONT, bool DOWN, bool GUARD>
+template <int CI, int CO, bool HASB, bool FF2, int NPOST, bool PASS, bool PRE, bool FRONT, bool DOWN, bool GUARD, bool RESTART = false>
 __global__ void __launch_bounds__(LANES_THREADS) k_fused_lanes(lanes::Args a) {
     extern __shared__ __align__(16) float lanes_smem[];
     const uint32_t warp = threadIdx.x >> 5;
     const uint32_t group = blockIdx.x * LANES_WARPS + warp;
     if (group >= a.n_groups) return;   // whole warps leave: the warp program only synchronises within a warp
-    lanes::warp_main<CI, CO, HASB, FF2, NPOST, PASS, PRE, FRONT, DOWN, GUARD>(a, group, lanes_smem + (size_t)warp * 32 * lanes::Geo<CI, DOWN ? lanes::NSLOT_DOWN : RB_LANES_UP_SLOTS>::RS);
+    lanes::warp_main<CI, CO, HASB, FF2, NPOST, PASS, PRE, FRONT, DOWN, GUARD, RESTART>(a, group, lanes_smem + (size_t)warp * 32 * lanes::Geo<CI, DOWN ? lanes::NSLOT_DOWN : RB_LANES_UP_SLOTS>::RS);
 }
 
 // The lane-pair kernel (rb_duo_core.h): a warp = 64 mono streams, two per lane sharing one index state.
@@ -358,7 +358,32 @@ static void launch_lanes_cc(const lanes::Args& a, bool has_biquad, bool ff2, boo
     else has_pre ? launch_lanes_c<CI, CO, false, true>(a, has_biquad, ff2, has_post, st) : launch_lanes_c<CI, CO, false, false>(a, has_biquad, ff2, has_post, st);
 }
 
+// The RESTART twins (rb_lanes_core.h: Cut).  One per (layout, filter, FRONT, DOWN): the twin of an up-sampling class is the
+// guarded PRE tile, and every twin takes plain coefficients and applies Row::post -- a gain of 1.0, the guard and the three-product
+// feed-forward give the bits of the variants they stand in for, and a class only comes here for the blocks that hold a cut.
+template <int CI, int CO>
+static void launch_restart_cc(const lanes::Args& a, bool has_biquad, bool front, cudaStream_t st) {
+    const uint32_t n_ctas = (a.n_groups + LANES_WARPS - 1) / LANES_WARPS;
+    const bool down = lanes::ratio_runs_down(a.from, a.to);
+#define RB_RESTART(HASB, PRE, FRONT, DOWN, GUARD) \
+    k_fused_lanes<CI, CO, HASB, false, 1, false, PRE, FRONT, DOWN, GUARD, true><<<n_ctas, LANES_THREADS, lanes_smem_bytes<CI, DOWN>(), st>>>(a)
+    if (front) down ? RB_RESTART(true, false, true, true, false) : RB_RESTART(true, false, true, false, false);
+    else if (down) has_biquad ? RB_RESTART(true, false, false, true, false) : RB_RESTART(false, false, false, true, false);
+    else has_biquad ? RB_RESTART(true, true, false, false, true) : RB_RESTART(false, true, false, false, true);
+#undef RB_RESTART
+}
+
 }  // namespace
+
+cudaError_t rb_lanes_launch_restart(const lanes::Args& a, uint32_t ch_in, uint32_t ch_out, bool has_biquad, bool front, cudaStream_t st) {
+    if (a.mix_len == 0 || a.n_groups == 0) return cudaSuccess;
+    if (!a.cuts || a.from == a.to || (front && !has_biquad)) return cudaErrorInvalidValue;
+    if (!((ch_in == 1 || ch_in == 2) && (ch_in == ch_out || (ch_in == 1 && ch_out == 2)))) return cudaErrorInvalidValue;
+    if (ch_in == 2) launch_restart_cc<2, 2>(a, has_biquad, front, st);
+    else if (ch_out == 2) launch_restart_cc<1, 2>(a, has_biquad, front, st);
+    else launch_restart_cc<1, 1>(a, has_biquad, front, st);
+    return cudaGetLastError();
+}
 
 cudaError_t rb_lanes_launch_kernel(const lanes::Args& a, uint32_t ch_in, uint32_t ch_out, bool has_biquad, bool ff2, bool has_post,
                                    bool has_pre, bool front, bool guard, cudaStream_t st) {

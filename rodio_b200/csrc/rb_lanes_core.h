@@ -96,6 +96,8 @@ struct Row {                 // one stream (whole, or the part of it one block o
     uint64_t n_int;          // outputs [0, n_int) interpolate between two frames (left frame <= L-2)
     uint64_t o0;             // streaming: stream-absolute index of the first output of the block (0 for whole streams)
     uint64_t i0;             // streaming: stream-absolute index of the frame at in[0]; (o0 * from) / to >= i0
+                             // (a session with restart schedules counts o0 and i0 from the first output and the first frame of the
+                             // row's converter run: i0 is then taken modulo 2^64, in[0] may lie in front of the run)
     float* state;            // streaming: per channel {x[n-1], x[n-2], y[n-1], y[n-2]} (4*C floats) read at the start,
                              // written at the end; NULL: start from zeros, keep nothing
     float b0, b1, b2, a1, a2;
@@ -109,6 +111,18 @@ struct Row {                 // one stream (whole, or the part of it one block o
                              // has consumed them; the gain in front (PRE: pre, FRONT: mid) applies to frames >= f0 only ...
     float ga, gb;            // ... frame f0 - 2 was pulled with gain ga, frame f0 - 1 with gb (Player::set_volume between blocks:
                              // a frame keeps the factor it was multiplied with when Amplify::next pulled it)
+};
+
+// RESTART (streaming sessions): the converter run of the row ends inside the block and the next one begins -- rodio's
+// UniformSourceIterator bootstraps a fresh SampleRateConverter there (src/source/uniform.rs:83-96), which interpolates inside
+// itself only, emits its last frame raw and starts again at numerator 0 with two new frames.  The Row describes the run that
+// ends (L, n_int, o0, i0 up to its last frame); from block-local output m on the lane walks the new run.  Filter state and gains
+// pass through; a filter in FRONT consumes every input frame once, in order, across the cut.
+struct Cut {
+    uint64_t m;              // first output of the new run, relative to Row::mix_start; >= Row::out_len: no cut in this block
+    uint64_t n_int;          // of the outputs [m, out_len) the first n_int interpolate
+    uint64_t i0;             // Row::i0 of the new run, whose o0 is 0: its first frame is in[-i0] (modulo 2^64)
+    uint64_t L;              // Row::L of the new run
 };
 
 // Optional per-group record (duo kernel, time-parallel plan): which partial row the group adds into, and from which timeline
@@ -133,6 +147,7 @@ struct Args {
     const float* zeros;      // CHUNK zeros, 16-byte aligned: the source of idle lanes
     const uint32_t* unsafe;  // optional [n_rows]: non-zero = as if ROW_UNSAFE were set (streaming: kept on the device)
     const GroupSpan* spans;  // optional [n_groups] (rb_duo_core.h)
+    const Cut* cuts;         // RESTART: [n_rows]
 };
 
 // (t - a1*y1) - a2*y2, each product and each difference rounded once (src/source/blt.rs:558-560)
@@ -177,14 +192,19 @@ SIMT_FN float reduce_tile(const float (&v)[TILE], uint32_t ln) {
 // applied (no PRE twin).  Larger ratios stay on the slow tiles.  With FRONT the one or two frames an output moves on are
 // one or two steps of the filter.
 //
+// RESTART: rows may change their converter run once inside the block (Cut above).  The tile that holds a lane's cut is a slow
+// tile -- the ending run's fast tiles stop where its interpolating outputs do -- whose closed form switches to the new run at
+// the cut; the fast run behind it is primed from the new run's (o0 = 0, i0).
+//
 // GUARD (with PRE): some stream of the class has a gain in front outside [2^-6, 2^6] (a Player at -40 dB): its scaled taps may
 // leave the range in which the reciprocal division is exact, so the tile checks every quotient like FRONT does and the
 // stream stays on the fast tiles.  The host picks the variant per launch; rows and their order are the same, and so are the
 // bits of every stream whose quotients were in range anyway.
 template <int CI, int CO, bool HASB, bool FF2, int NPOST, bool PASS = false, bool PRE = false, bool FRONT = false, bool DOWN = false,
-          bool GUARD = false>
+          bool GUARD = false, bool RESTART = false>
 SIMT_FN void warp_main(const Args& a, uint32_t group, float* ring_warp) {
     static_assert(!GUARD || (PRE && !PASS), "GUARD: the guarded twin of the interpolating PRE variant");
+    static_assert(!RESTART || !PASS, "RESTART: a same-rate conversion keeps nothing across a restart");
     static_assert(CI == CO || (CI == 1 && CO == 2), "channel layouts served");
     static_assert(!DOWN || (!PASS && !PRE), "DOWN: interpolating, the gain in front always applied");
     static_assert(!FRONT || (HASB && !FF2 && !PRE), "FRONT: plain coefficients, the gain in front is always applied");
@@ -204,13 +224,14 @@ SIMT_FN void warp_main(const Args& a, uint32_t group, float* ring_warp) {
         row.in = a.zeros, row.L = 0, row.out_len = 0, row.mix_start = 0, row.n_int = 0, row.o0 = 0, row.i0 = 0, row.state = nullptr;
         row.b0 = row.b1 = row.b2 = row.a1 = row.a2 = row.ffk = row.post = row.pre = row.mid = row.ga = row.gb = 0.0f, row.flags = 0, row.f0 = 0;
     }
-    const uint64_t ms = row.mix_start, end = row.mix_start + row.out_len;   // frames
+    uint64_t ms = row.mix_start, end = row.mix_start + row.out_len;   // frames; RESTART: of the run the lane is in
+    uint64_t L = row.L, n_int = row.n_int;
     // Down-sampling classes (from > to: more than one input frame per output) are served by the slow tiles only -- exact,
     // general, not fast; the fast run below assumes at most one new frame per step.
     // (a same-rate stream never divides, a guarded tile checks every quotient: ROW_FORCE_SLOW means nothing to them)
     const bool safe = has && (a.from <= a.to || (DOWN && a.from <= 2 * a.to)) && (PASS || GUARD || !(row.flags & ROW_FORCE_SLOW)) &&
                       (PASS || FRONT || (!(row.flags & ROW_UNSAFE) && !(a.unsafe && a.unsafe[r])));
-    const bool stops = !(row.flags & ROW_CONTINUES);   // the stream ends inside this block (or is a whole stream)
+    bool stops = !(row.flags & ROW_CONTINUES);   // the stream ends inside this block (or is a whole stream)
     const bool live = has && row.out_len != 0;
     const uint64_t t_lo = simt::reduce_min64(live ? ms : ~0ull), t_hi = simt::reduce_max64(live ? end : 0ull);
     if (t_lo >= t_hi) return;
@@ -236,7 +257,22 @@ SIMT_FN void warp_main(const Args& a, uint32_t group, float* ring_warp) {
     }
     // stream-absolute numerator of local output frame o is (o0 + o) * from; the input frame it falls on, relative to
     // in[0], is that / to - i0.  Both offsets are zero for whole streams.
-    const uint64_t o0 = row.o0, i0 = row.i0;
+    uint64_t o0 = row.o0, i0 = row.i0;
+    // RESTART: the lane walks the ending run up to timeline frame cut_t and moves to the new one when it gets there
+    Cut cut;
+    uint64_t cut_t = ~0ull;
+    if (RESTART && has && a.cuts[r].m < row.out_len) {
+        cut = a.cuts[r];
+        cut_t = ms + cut.m;
+        end = cut_t, stops = false;
+    }
+    auto restart_at = [&](uint64_t tt) {
+        if (RESTART && tt >= cut_t) {
+            ms = cut_t, end = row.mix_start + row.out_len, stops = !(row.flags & ROW_CONTINUES);
+            o0 = 0, i0 = cut.i0, L = cut.L, n_int = cut.n_int;
+            cut_t = ~0ull;
+        }
+    };
     const uint32_t cq = ln % QPC;                      // the quad of a chunk this lane copies ...
     const uint32_t cr = ln / QPC;                      // ... for stream cr + RPI * j of the warp
     // FRONT: one step of the filter on input frame `raw` (src/source/blt.rs:397-410 on src/source/amplify.rs:91-95)
@@ -261,6 +297,7 @@ SIMT_FN void warp_main(const Args& a, uint32_t group, float* ring_warp) {
     };
 
     while (t < t_end) {
+        restart_at(t);
         // ---- how long does every lane stay "interior or idle" from t on? ----
         uint32_t d;
         if (!has || t >= end) {
@@ -277,7 +314,7 @@ SIMT_FN void warp_main(const Args& a, uint32_t group, float* ring_warp) {
             d = 0;
             // FRONT: the index step behind the last output of a run already feeds the NEXT frame to the filter, so that
             // output must be an interpolating one as well (its right neighbour exists): the run stops one output short
-            const uint64_t n_fast = FRONT ? (row.n_int ? row.n_int - 1 : 0) : row.n_int;
+            const uint64_t n_fast = FRONT ? (n_int ? n_int - 1 : 0) : n_int;
             if (safe && o + TF <= n_fast) {
                 const uint64_t g = (n_fast - o) / TF * TF;
                 d = g > RUN_CAP ? RUN_CAP : (uint32_t)g;
@@ -301,7 +338,7 @@ SIMT_FN void warp_main(const Args& a, uint32_t group, float* ring_warp) {
                 const uint64_t ibase = i & ~3ull;       // a multiple of 4 frames: 16-byte aligned for either C
                 k0 = (uint32_t)(i - ibase);
                 src = row.in + ibase * C;
-                const uint64_t mq = ((row.L * C - 1) >> 2) - ((ibase * C) >> 2);   // last quad (relative) that holds a frame
+                const uint64_t mq = ((L * C - 1) >> 2) - ((ibase * C) >> 2);   // last quad (relative) that holds a frame
                 maxq = mq > 0x7fffffffull ? 0x7fffffffu : (uint32_t)mq;
                 if (FRONT) front_catch_up(i + 2);       // interior: i + 1 < L
                 if (PRE || FRONT || DOWN) g_tap0 = gain_of(i), g_tap1 = gain_of(i + 1);
@@ -499,6 +536,7 @@ SIMT_FN void warp_main(const Args& a, uint32_t group, float* ring_warp) {
 #pragma unroll 1
             for (int f = 0; f < TF; f++) {
                 const uint64_t tt = t + (uint64_t)f;
+                restart_at(tt);
                 const bool on = has && tt >= ms && tt < end;
                 uint64_t i = 0;
                 uint32_t num = 0;
@@ -511,7 +549,7 @@ SIMT_FN void warp_main(const Args& a, uint32_t group, float* ring_warp) {
 #pragma unroll
                     for (int c = 0; c < C; c++) xh1[c] = xh2[c] = y1[c] = y2[c] = 0.f;
                 }
-                if (FRONT && on) front_catch_up(i + 2 < row.L ? i + 2 : row.L);
+                if (FRONT && on) front_catch_up(i + 2 < L ? i + 2 : L);
                 float val[C];
 #pragma unroll
                 for (int c = 0; c < C; c++) {
@@ -529,7 +567,7 @@ SIMT_FN void warp_main(const Args& a, uint32_t group, float* ring_warp) {
                         float xa = simt::ldg(row.in + i * C + c);
                         if (PRE || DOWN) xa = simt::fmul(xa, gain_of(i));
                         float x = xa;
-                        if (!PASS && i + 1 < row.L) {
+                        if (!PASS && i + 1 < L) {
                             float xb = simt::ldg(row.in + (i + 1) * C + c);
                             if (PRE || DOWN) xb = simt::fmul(xb, gain_of(i + 1));
                             x = simt::fadd(xa, simt::fdiv(simt::fmul(simt::fsub(xb, xa), simt::u2f(num)), den));

@@ -4,8 +4,49 @@
 // keeps running there; the CUDA build launches the kernels instead.  Same jobs, same order of the additions, one sample at a
 // time.  The translation unit is compiled with -ffp-contract=off, like the kernels.
 #pragma once
+#include <limits>
+#include <utility>
+#include <vector>
+
 #include "rb_lanes.h"
 #include "rb_lanes_plan.h"
+
+// The RESTART twins of the lane kernel (rb_lanes.cu: launch_restart_cc) on the SIMT emulator.  The session lists what its kernels
+// may read (its own device buffers) in g_restart_readable before the launch; the ring starts out as NaN, so a cursor seeded wrongly
+// behind a cut shows.
+namespace session_host {
+inline std::vector<std::pair<const char*, const char*>> g_restart_readable;
+template <int CI, int CO, bool HASB, bool PRE, bool FRONT, bool DOWN, bool GUARD>
+void restart_group(const lanes::Args& a, uint32_t g, simt::WarpEmu* w, float* ring) {
+    simt::run_warp(w, [&] { lanes::warp_main<CI, CO, HASB, false, 1, false, PRE, FRONT, DOWN, GUARD, true>(a, g, ring); });
+}
+template <int CI, int CO>
+void restart_cc(const lanes::Args& a, uint32_t g, simt::WarpEmu* w, float* ring, bool has_biquad, bool front) {
+    const bool down = lanes::ratio_runs_down(a.from, a.to);
+    if (front) down ? restart_group<CI, CO, true, false, true, true, false>(a, g, w, ring) : restart_group<CI, CO, true, false, true, false, false>(a, g, w, ring);
+    else if (down) has_biquad ? restart_group<CI, CO, true, false, false, true, false>(a, g, w, ring) : restart_group<CI, CO, false, false, false, true, false>(a, g, w, ring);
+    else has_biquad ? restart_group<CI, CO, true, true, false, false, true>(a, g, w, ring) : restart_group<CI, CO, false, true, false, false, true>(a, g, w, ring);
+}
+}  // namespace session_host
+
+cudaError_t rb_lanes_launch_restart(const lanes::Args& a, uint32_t ch_in, uint32_t ch_out, bool has_biquad, bool front, cudaStream_t) {
+    if (a.mix_len == 0 || a.n_groups == 0) return cudaSuccess;
+    if (!a.cuts || a.from == a.to || (front && !has_biquad)) return cudaErrorInvalidValue;
+    if (!((ch_in == 1 || ch_in == 2) && (ch_in == ch_out || (ch_in == 1 && ch_out == 2)))) return cudaErrorInvalidValue;
+    simt::WarpEmu warp;
+    warp.readable = session_host::g_restart_readable;
+    constexpr int MAX_RS = lanes::Geo<2, 4>::RS;   // the largest ring of any variant
+    std::vector<float> ring_store(32 * MAX_RS + 4);
+    float* ring = ring_store.data();
+    while ((uintptr_t)ring & 15) ring++;
+    for (uint32_t g = 0; g < a.n_groups; g++) {
+        for (int i = 0; i < 32 * MAX_RS; i++) ring[i] = std::numeric_limits<float>::quiet_NaN();
+        if (ch_in == 2) session_host::restart_cc<2, 2>(a, g, &warp, ring, has_biquad, front);
+        else if (ch_out == 2) session_host::restart_cc<1, 2>(a, g, &warp, ring, has_biquad, front);
+        else session_host::restart_cc<1, 1>(a, g, &warp, ring, has_biquad, front);
+    }
+    return cudaSuccess;
+}
 
 cudaError_t rb_lanes_fifo_scatter(const float* staging, const rb_fifo_job* jobs, uint32_t n_jobs, float* fifo, uint64_t stride,
                                   uint32_t* flags, cudaStream_t) {

@@ -14,6 +14,11 @@
 //   * biquad: x[n-1], x[n-2], y[n-1], y[n-2] (src/source/blt.rs:397-410) -- four floats per stream on the device; a filter
 //     in FRONT of the conversion additionally has a position of its own in the input (Stream::fpos): it has consumed the
 //     right neighbour of the last output already, so its two last outputs are the interpolation taps.
+//   * restarts (RB_SESSION_RESTARTS): UniformSourceIterator does not convert a source as one run.  At every bootstrap it asks
+//     current_span_len(), caps it at 32768 samples and builds a fresh SampleRateConverter over that many samples
+//     (src/source/uniform.rs:50-68, :83-96); the run pulls its first two frames at once, interpolates inside itself only and emits
+//     its last frame raw.  A stream with a schedule keeps the run the next output belongs to -- its first input and output frame --
+//     and the ends of the runs the pushes have begun; everything above applies to each run with indices relative to its start.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -36,6 +41,13 @@ struct Stream {
                                // neighbour of the last output -- a gain in front of the conversion is final for them
     bool front = false;        // the source's filter sits in front of the conversion, runs once per INPUT frame and has
                                // consumed exactly those frames: the FIFO must keep everything from fpos on
+    // ---- restart schedule; run_cap == 0: none, the source is one run (every session without RB_SESSION_RESTARTS) ----
+    uint64_t run_cap = 0;      // frames a run holds at most: min(span_len, 32768) samples
+    uint64_t run_i = 0;        // the run of output `out_done`: its first input frame ...
+    uint64_t run_o = 0;        // ... and its first output frame (stream-absolute)
+    uint64_t sched_end = 0;    // input frame at which the run the pushes are filling ends (0: nothing pushed yet)
+    uint64_t runs_done = 0;    // runs played out
+    std::vector<uint64_t> ends;   // ends (input frame) of the runs begun by a push and not played out: ends[0] is the current run's
     uint64_t fill() const { return pushed - i0; }   // frames in the FIFO
 };
 
@@ -51,11 +63,50 @@ inline uint64_t out_total(uint64_t L, uint32_t from, uint32_t to) {
 inline uint64_t out_interp(uint64_t L, uint32_t from, uint32_t to) {
     return L < 2 ? 0 : ((L - 1) * (uint64_t)to + from - 1) / from;
 }
-// Output frames of stream `s` that exist so far (renderable): everything once it has ended, else the interpolated ones.
-inline uint64_t out_ready(const Stream& s) {
-    return s.eof ? out_total(s.pushed, s.from, s.to) : out_interp(s.pushed, s.from, s.to);
+// A push of n frames (PCM, or a pause's silence: real = false) is about to move `pushed`: the runs whose first frame is among
+// them begin.  A run's length is known when it begins -- run_cap, or what the source's take still lets through at that moment
+// (take_left frames, ~0: no take; src/source/take.rs:180-196), the silence inside the run counted against it as rodio's Take
+// counts Pausable's zeros.
+inline void schedule_push(Stream& s, uint64_t n, uint64_t take_left, bool real) {
+    if (!s.run_cap) return;
+    for (uint64_t at = s.pushed, stop = s.pushed + n; at < stop;) {
+        if (at == s.sched_end) s.sched_end = at + std::min(s.run_cap, take_left), s.ends.push_back(s.sched_end);
+        const uint64_t step = std::min(stop, s.sched_end) - at;
+        if (real && take_left != ~0ull) take_left -= step;
+        at += step;
+    }
 }
-inline bool finished(const Stream& s) { return s.eof && s.out_done >= out_total(s.pushed, s.from, s.to); }
+// Output frames of stream `s` that exist so far (renderable): everything once it has ended, else the interpolated ones.  With a
+// schedule, run by run: a run whose last frame has arrived is complete, its raw last frame included, whatever follows.
+inline uint64_t out_ready(const Stream& s) {
+    if (!s.run_cap) return s.eof ? out_total(s.pushed, s.from, s.to) : out_interp(s.pushed, s.from, s.to);
+    uint64_t i = s.run_i, o = s.run_o;
+    for (uint64_t e : s.ends) {
+        const uint64_t L = std::min(s.pushed, e) - i;
+        if (s.pushed < e && !s.eof) return o + out_interp(L, s.from, s.to);
+        o += out_total(L, s.from, s.to), i = e;
+    }
+    return o;
+}
+// All of the stream's output frames, once it has its end of stream.
+inline uint64_t out_end(const Stream& s) { return s.run_cap ? out_ready(s) : out_total(s.pushed, s.from, s.to); }
+inline bool finished(const Stream& s) { return s.eof && s.out_done >= out_end(s); }
+// Moves to the run of output `out_done`: runs that are complete and played out are left behind.
+inline void settle(Stream& s) {
+    while (!s.ends.empty() && (s.pushed >= s.ends[0] || s.eof)) {
+        const uint64_t e = std::min(s.pushed, s.ends[0]), n = out_total(e - s.run_i, s.from, s.to);
+        if (s.out_done < s.run_o + n) break;
+        s.run_i = e, s.run_o += n, s.runs_done++;
+        s.ends.erase(s.ends.begin());
+    }
+}
+// Converter runs that have produced an output so far.
+inline uint64_t runs_started(const Stream& s) { return s.runs_done + (s.out_done > s.run_o ? 1 : 0); }
+// A block renders at most one restart per stream: the timeline frame up to which a block may go (after settle).
+inline uint64_t one_cut_limit(const Stream& s) {
+    if (s.ends.size() < 3) return ~0ull;
+    return s.mix_start + s.run_o + out_total(s.ends[0] - s.run_i, s.from, s.to) + out_total(s.ends[1] - s.ends[0], s.from, s.to);
+}
 
 // How many mixer frames [T, T + n) can be rendered now (every unfinished stream must be able to supply its part).
 // Returns 0 with *ended = true when no stream is left (MixerSource::next returns None, src/mixer.rs:129-135).
@@ -71,7 +122,7 @@ inline void resolve_queue(std::vector<Stream>& st, uint64_t T) {
             if (!s.held || s.follows < 0) continue;
             const Stream& p = st[(size_t)s.follows];
             if (p.held || !p.eof) continue;
-            s.mix_start = std::max(T, p.mix_start + out_total(p.pushed, p.from, p.to));
+            s.mix_start = std::max(T, p.mix_start + out_end(p));
             s.held = false, again = true;
         }
     }
@@ -98,10 +149,17 @@ inline uint64_t renderable(const std::vector<Stream>& st, uint64_t T, uint64_t m
 struct Part {
     uint64_t mix_start = 0;   // block-local timeline position of its first output
     uint64_t out_len = 0;     // outputs it contributes
-    uint64_t o0 = 0;          // stream-absolute index of the first of them
-    uint64_t n_int = 0;       // how many of them interpolate (the rest is the raw last frame)
+    uint64_t o0 = 0;          // index of the first of them in its converter run (stream-absolute without a schedule)
+    uint64_t n_int = 0;       // how many of them interpolate (the rest is the raw last frame); with a cut: of those in front of it
     bool continues = false;   // more outputs will follow in later blocks
+    uint64_t o_abs = 0;       // stream-absolute index of the first output
+    uint64_t run_i = 0;       // first input frame of the run of o0 (stream-absolute) ...
+    uint64_t run_end = 0;     // ... and the frame behind the last one of it that has arrived
+    // the block's restart: outputs [cut_m, out_len) belong to the next run (cut_m == out_len: none), which begins at input frame
+    // cut_i, has frames up to cut_end so far and interpolates on its first cut_n_int outputs
+    uint64_t cut_m = 0, cut_i = 0, cut_end = 0, cut_n_int = 0;
 };
+// (after settle; a block stays within one_cut_limit of every stream)
 inline Part part_of(const Stream& s, uint64_t T, uint64_t n) {
     Part p;
     if (s.held) {
@@ -115,10 +173,19 @@ inline Part part_of(const Stream& s, uint64_t T, uint64_t n) {
         p.continues = !finished(s);
         return p;
     }
-    p.mix_start = lo - T, p.out_len = hi - lo, p.o0 = lo - s.mix_start;
-    const uint64_t ni = out_interp(s.pushed, from, to);
+    p.mix_start = lo - T, p.out_len = p.cut_m = hi - lo, p.o_abs = lo - s.mix_start;
+    p.run_i = s.run_i, p.run_end = s.run_cap ? std::min(s.pushed, s.ends[0]) : s.pushed;
+    p.o0 = p.o_abs - s.run_o;
+    const uint64_t ni = out_interp(p.run_end - p.run_i, from, to);
     p.n_int = ni > p.o0 ? std::min(p.out_len, ni - p.o0) : 0;
-    p.continues = !(s.eof && p.o0 + p.out_len >= out_total(s.pushed, from, to));
+    p.continues = !(s.eof && p.o_abs + p.out_len >= ready);
+    if (s.run_cap && s.ends.size() > 1) {   // the current run is complete: does the block go past its last output?
+        const uint64_t run_out = out_total(p.run_end - p.run_i, from, to);
+        if (p.o0 + p.out_len > run_out) {
+            p.cut_m = run_out - p.o0, p.cut_i = s.ends[0], p.cut_end = std::min(s.pushed, s.ends[1]);
+            p.cut_n_int = std::min(p.out_len - p.cut_m, out_interp(p.cut_end - p.cut_i, from, to));
+        }
+    }
     return p;
 }
 // Mixer::add for a held source while the mixer has rendered T frames: it joins at the next frame (src/mixer.rs:175-183).
@@ -133,16 +200,21 @@ inline void skip(Stream& s) {
     s.pushed = std::min(s.pushed, std::max(s.fpos, s.i0));
     s.eof = true;
     if (s.held) s.held = false, s.follows = -1, s.pushed = s.i0 = s.fpos = 0, s.out_done = 0, s.mix_start = 0;
+    size_t keep = 0;           // runs none of whose frames is left never begin
+    for (uint64_t i = s.run_i; keep < s.ends.size() && i < s.pushed; i = s.ends[keep++]) {}
+    s.ends.resize(keep);
 }
 
 // After the block: advance the stream and tell how many FIFO frames (from the front) are dead.
 inline uint64_t advance(Stream& s, const Part& p) {
     if (p.out_len) {   // the converter (and a filter in front of it) stands behind the right neighbour of the block's last output
-        const uint64_t ia = ((p.o0 + p.out_len - 1) * (uint64_t)s.from) / s.to;
-        s.fpos = std::min(ia + 2, s.pushed);
+        const bool cut = p.cut_m < p.out_len;   // ... in the run of that output: a new run pulls its first two frames at once
+        const uint64_t ia = ((cut ? p.out_len - 1 - p.cut_m : p.o0 + p.out_len - 1) * (uint64_t)s.from) / s.to;
+        s.fpos = std::min((cut ? p.cut_i : p.run_i) + ia + 2, cut ? p.cut_end : p.run_end);
     }
-    s.out_done = p.out_len ? p.o0 + p.out_len : s.out_done;
-    uint64_t left = std::min((s.out_done * (uint64_t)s.from) / s.to, s.pushed);   // left frame of the next output
+    s.out_done = p.out_len ? p.o_abs + p.out_len : s.out_done;
+    settle(s);
+    uint64_t left = std::min(s.run_i + ((s.out_done - s.run_o) * (uint64_t)s.from) / s.to, s.pushed);   // left frame of the next output
     if (s.front) left = std::min(left, s.fpos);   // more than two input frames per output: the filter still needs the ones between
     const uint64_t keep_from = left & ~3ull;                                        // FIFO front stays 16-byte aligned
     const uint64_t drop = keep_from > s.i0 ? keep_from - s.i0 : 0;

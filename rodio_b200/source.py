@@ -700,8 +700,10 @@ class Session:
 
     def __init__(self, sources: Sequence[Source], mixer_rate: int, fifo_frames: int = 8192, max_block_frames: int = 4096,
                  mix_starts: Optional[Sequence[int]] = None, ctx: Optional[Context] = None, mixer_channels: Optional[int] = None,
-                 master: Sequence[Effect] = ()):
-        """master: adapters on the mixer's output, [amplify] [limit] [amplify] (rb_session_set_master)."""
+                 master: Sequence[Effect] = (), restarts: bool = False):
+        """master: adapters on the mixer's output, [amplify] [limit] [amplify] (rb_session_set_master).
+        restarts: RB_SESSION_RESTARTS -- the mixer's conversion restarts where rodio's does: every min(span_len, 32768) samples of
+        a source that reports a span (a SamplesBuffer reports its length), and behind take_duration (include/rodio_b200.h)."""
         self.ctx = ctx or default_context()
         self.sources = list(sources)
         self.max_block_frames = max_block_frames
@@ -710,8 +712,12 @@ class Session:
         self.src_channels = [s.base_channels for s in self.sources]       # what is pushed: the source's own interleaving
         self._descs, self._keep = pack_descs(self.sources, mix_starts)
         self._h = C.c_void_p()
-        check(lib().rb_session_create(self.ctx._h, self.channels, mixer_rate, self._descs, len(self.sources), fifo_frames,
-                                      max_block_frames, C.byref(self._h)), "rb_session_create")
+        if restarts:
+            check(lib().rb_session_create_ex(self.ctx._h, self.channels, mixer_rate, self._descs, len(self.sources), fifo_frames,
+                                             max_block_frames, capi.RB_SESSION_RESTARTS, C.byref(self._h)), "rb_session_create_ex")
+        else:
+            check(lib().rb_session_create(self.ctx._h, self.channels, mixer_rate, self._descs, len(self.sources), fifo_frames,
+                                          max_block_frames, C.byref(self._h)), "rb_session_create")
         if master:
             try:
                 self.set_master(master)
@@ -774,6 +780,18 @@ class Session:
         """Player::set_volume (src/player.rs:180-186): the AMPLIFY in FRONT of the mixer's conversion (behind a filter in front
         of it, where the Player keeps its own, src/player.rs:120-128), for every frame the converter pulls from now on."""
         check(lib().rb_session_set_volume(self._h, stream, float(factor)), "rb_session_set_volume")
+
+    def source_runs(self, stream: int) -> int:
+        """Converter runs of the source that have produced an output so far (rb_session_source_runs)."""
+        n = C.c_uint64()
+        check(lib().rb_session_source_runs(self._h, stream, C.byref(n)), "rb_session_source_runs")
+        return n.value
+
+    def restart_launches(self) -> int:
+        """Launches of the lane kernel's RESTART variants so far: only blocks in which a source restarts make one."""
+        n = C.c_uint64()
+        check(lib().rb_session_restart_launches(self._h, C.byref(n)), "rb_session_restart_launches")
+        return n.value
 
     def available(self) -> Tuple[int, bool]:
         n, e = C.c_uint64(), C.c_int()
