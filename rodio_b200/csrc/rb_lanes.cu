@@ -101,12 +101,15 @@ __global__ void __launch_bounds__(256) k_lerp_mix(rb_lerpmix_args a) {
     uint32_t tap[LM_U], pos[LM_U];     // tap: left input frame of the position, relative to the tile's first
     float numf[LM_U], acc[LM_U];
     bool any[LM_U];
-    const uint64_t i_tile = ((tile_lo - a.origin) * (uint64_t)a.from) / a.to;   // origin <= every position that any stream covers
-    const uint32_t n_win = (uint32_t)((((tile_hi - 1 - a.origin) * (uint64_t)a.from) / a.to) - i_tile) + 2;   // frames a full row needs
+    // origin <= every position that any stream covers, and origin need not be a multiple of the tile: the tile's taps start at
+    // base, and a position in front of it (no stream covers it) takes base's tap, so that no subtraction below wraps around
+    const uint64_t base = max(tile_lo, a.origin);
+    const uint64_t i_tile = ((base - a.origin) * (uint64_t)a.from) / a.to;
+    const uint32_t n_win = (uint32_t)((((max(tile_hi - 1, base) - a.origin) * (uint64_t)a.from) / a.to) - i_tile) + 2;   // frames a full row needs
 #pragma unroll
     for (int u = 0; u < LM_U; u++) {
         const uint64_t n = tile_lo + (uint64_t)u * 256 + threadIdx.x;
-        const uint64_t prod = (n - a.origin) * (uint64_t)a.from;
+        const uint64_t prod = (max(n, base) - a.origin) * (uint64_t)a.from;
         const uint64_t i = prod / a.to;
         tap[u] = (uint32_t)(i - i_tile), numf[u] = __uint2float_rn((uint32_t)(prod - i * a.to)), pos[u] = (uint32_t)n;
         acc[u] = 0.0f, any[u] = false;
