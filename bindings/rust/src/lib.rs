@@ -295,6 +295,10 @@ impl Source for GpuMixerSource {
 // in the session, so the block size is free -- 10 ms blocks for a cpal callback, whole seconds for offline renders.
 pub enum rb_session {}
 pub const RB_SESSION_RESTARTS: u32 = 1;
+/// What `current_span_len()` starts to return during a push: after `at` samples of the push (0 = None).
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct rb_span_mark { pub at: u64, pub span_len: u32, pub pad_: u32 }
 #[repr(C)]
 pub struct rb_wav_info { pub sample_rate: u32, pub channels: u16, pub bits_per_sample: u16, pub format: u16, pub packed24: u16, pub pad_: u32,
                          pub data_offset: u64, pub data_bytes: u64, pub n_samples: u64 }
@@ -311,6 +315,11 @@ extern "C" {
     fn rb_session_destroy(s: *mut rb_session) -> i32;
     fn rb_session_push_packed(s: *mut rb_session, pcm: *const f32, n_frames: *const u64, end_of_stream: *const u8) -> i32;
     fn rb_session_push_silence(s: *mut rb_session, stream: usize, n_frames: u64) -> i32;
+    /// `rb_session_push` / `rb_session_push_packed` with span marks (sessions created with `RB_SESSION_RESTARTS`).
+    pub fn rb_session_push_spans(s: *mut rb_session, stream: usize, pcm: *const f32, n_frames: u64, marks: *const rb_span_mark,
+                                 n_marks: u32, end_of_stream: i32) -> i32;
+    fn rb_session_push_packed_spans(s: *mut rb_session, pcm: *const f32, n_frames: *const u64, end_of_stream: *const u8,
+                                    n_marks: *const u32, marks: *const rb_span_mark) -> i32;
     fn rb_session_render(s: *mut rb_session, out: *mut f32, max_frames: u64, written: *mut u64, ended: *mut i32) -> i32;
     fn rb_session_follow(s: *mut rb_session, stream: usize, predecessor: usize) -> i32;
     fn rb_session_skip(s: *mut rb_session, stream: usize) -> i32;
@@ -333,9 +342,48 @@ pub struct GpuLiveMixer {
     pull_frames: usize,                    // input frames pulled per source and refill
     sample_rate: SampleRate,
     ended: bool,
+    // `new_following_spans` only: per source, the last report seen and the changes not pushed yet (samples into the next push)
+    reports: Option<Vec<Option<usize>>>,
+    pending: Vec<Vec<rb_span_mark>>,
 }
 
 impl GpuLiveMixer {
+    /// A session over `descs` (one mono chain per input, see `rb_session_create`) fed by pulling `inputs`, `pull_frames` samples
+    /// per source and refill.  The conversion runs each source as one run.
+    pub fn new(ctx: *mut rb_context, descs: &[rb_stream_desc], inputs: Vec<Box<dyn Source + Send>>, pull_frames: usize,
+               sample_rate: SampleRate) -> Result<Self, i32> {
+        Self::create(ctx, descs, inputs, pull_frames, sample_rate, false)
+    }
+    /// The same with `RB_SESSION_RESTARTS`: the mixer's conversion restarts where rodio's `UniformSourceIterator` does, for any
+    /// source.  The shim records `current_span_len()` once before the first pull and after every pull, and pushes the changes as
+    /// span marks (`rb_session_push_packed_spans`) -- a decoder reports the packet it decoded last.
+    pub fn new_following_spans(ctx: *mut rb_context, descs: &[rb_stream_desc], inputs: Vec<Box<dyn Source + Send>>, pull_frames: usize,
+                               sample_rate: SampleRate) -> Result<Self, i32> {
+        Self::create(ctx, descs, inputs, pull_frames, sample_rate, true)
+    }
+    fn create(ctx: *mut rb_context, descs: &[rb_stream_desc], inputs: Vec<Box<dyn Source + Send>>, pull_frames: usize,
+              sample_rate: SampleRate, spans: bool) -> Result<Self, i32> {
+        let mut session: *mut rb_session = std::ptr::null_mut();
+        let rc = unsafe {
+            if spans {
+                rb_session_create_ex(ctx, 1, sample_rate.get(), descs.as_ptr(), descs.len(), (4 * pull_frames).max(4096) as u32, 4096,
+                                     RB_SESSION_RESTARTS, &mut session)
+            } else {
+                rb_session_create(ctx, 1, sample_rate.get(), descs.as_ptr(), descs.len(), (4 * pull_frames).max(4096) as u32, 4096, &mut session)
+            }
+        };
+        if rc != 0 { return Err(rc); }
+        let n = inputs.len();
+        // the report before the first pull goes first: a mark at 0 of the first push
+        let reports = if spans { Some(inputs.iter().map(|s| s.current_span_len()).collect::<Vec<_>>()) } else { None };
+        let pending = match &reports {
+            Some(r) => r.iter().map(|v| vec![rb_span_mark { at: 0, span_len: v.unwrap_or(0) as u32, pad_: 0 }]).collect(),
+            None => vec![Vec::new(); n],
+        };
+        Ok(GpuLiveMixer { session, inputs, done: vec![false; n], block: Vec::new(), at: 0, pull_frames, sample_rate, ended: false, reports,
+                          pending })
+    }
+
     /// `Player::pause` of input `stream` for `n_frames` frames: whole frames of 0.0 go to the mixer while the source (and any
     /// fade or take at the front of its chain) is not pulled -- `Pausable` (src/source/pausable.rs).  Returns the rb_status.
     pub fn push_silence(&mut self, stream: usize, n_frames: u64) -> i32 {
@@ -347,6 +395,8 @@ impl GpuLiveMixer {
         let mut pcm: Vec<f32> = Vec::with_capacity(self.inputs.len() * self.pull_frames);
         let mut n = vec![0u64; self.inputs.len()];
         let mut eos = vec![0u8; self.inputs.len()];
+        let mut marks: Vec<rb_span_mark> = Vec::new();
+        let mut n_marks = vec![0u32; self.inputs.len()];
         for (i, src) in self.inputs.iter_mut().enumerate() {
             if self.done[i] { continue; }
             for _ in 0..self.pull_frames {
@@ -354,12 +404,32 @@ impl GpuLiveMixer {
                     Some(s) => { pcm.push(s); n[i] += 1; }
                     None => { self.done[i] = true; eos[i] = 1; break; }
                 }
+                if let Some(r) = self.reports.as_mut() {      // a change seen after `n[i]` samples of this push
+                    let now = src.current_span_len();
+                    if now != r[i] {
+                        r[i] = now;
+                        let m = rb_span_mark { at: n[i], span_len: now.unwrap_or(0) as u32, pad_: 0 };
+                        match self.pending[i].last_mut() {
+                            Some(last) if last.at == m.at => *last = m,
+                            _ => self.pending[i].push(m),
+                        }
+                    }
+                }
+            }
+            if self.reports.is_some() {   // marks inside this push go now; one after its last sample waits for the next push (at 0)
+                let keep: Vec<rb_span_mark> = self.pending[i].iter().filter(|m| m.at >= n[i]).map(|m| rb_span_mark { at: 0, ..*m }).collect();
+                for m in self.pending[i].iter().filter(|m| m.at < n[i]) { marks.push(*m); n_marks[i] += 1; }
+                self.pending[i] = keep.into_iter().last().into_iter().collect();
             }
         }
         self.block.resize(4096, 0.0);
         let (mut written, mut ended) = (0u64, 0i32);
         unsafe {
-            rb_session_push_packed(self.session, pcm.as_ptr(), n.as_ptr(), eos.as_ptr());
+            if self.reports.is_some() {
+                rb_session_push_packed_spans(self.session, pcm.as_ptr(), n.as_ptr(), eos.as_ptr(), n_marks.as_ptr(), marks.as_ptr());
+            } else {
+                rb_session_push_packed(self.session, pcm.as_ptr(), n.as_ptr(), eos.as_ptr());
+            }
             rb_session_render(self.session, self.block.as_mut_ptr(), 4096, &mut written, &mut ended);
         }
         self.block.truncate(written as usize);

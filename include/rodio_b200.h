@@ -363,14 +363,16 @@ rb_status rb_session_create(rb_context* ctx, uint16_t mixer_channels, uint32_t m
  * 32768 samples and builds a fresh SampleRateConverter over that many samples, which interpolates inside itself only, emits its
  * last frame raw and starts again at numerator 0 (src/source/uniform.rs:50-68, src/conversions/sample_rate.rs:58-71, :187-199).
  * With the flag desc.span_len means what it means in batches: 0 = None, one run for the whole source; S > 0 = the source reports
- * Some(S) at every bootstrap (a SamplesBuffer: its length; a decoder: its packet), so runs are min(S, 32768) samples until the
- * input ends.  desc.n_samples stays ignored.  A resampled source whose push program holds a TAKE_DURATION restarts every
+ * Some(S) at every bootstrap (a SamplesBuffer: its length), so runs are min(S, 32768) samples until the input ends -- unless the
+ * pushes say that the report changes (rb_session_push_spans: a decoder reports the packet it decoded last).  desc.n_samples stays
+ * ignored.  A resampled source whose push program holds a TAKE_DURATION restarts every
  * min(samples left in the take, S, 32768) samples, the frames of rb_session_push_silence counted against the run as rodio's Take
  * counts Pausable's zeros: such takes may be longer than one run and may be paused.  Filter state and gains carry across a
  * restart, for any split into pushes and renders.  A source at the mixer's rate keeps no conversion state: its restarts change
  * nothing and are not tracked.  RB_ERR_UNSUPPORTED: a schedule whose runs are not whole frames of the source (span_len not a
  * multiple of its channel count; 3, 5, 6, 7 ... channels under the 32768 cap; a resampled take that ends inside a frame) and runs
- * shorter than two frames.  Such a session writes state blob version 8 when some source has a schedule. */
+ * shorter than two frames.  Such a session writes state blob version 8 when some source has a schedule, version 9 once a push
+ * carried span marks. */
 #define RB_SESSION_RESTARTS 1u
 rb_status rb_session_create_ex(rb_context* ctx, uint16_t mixer_channels, uint32_t mixer_sample_rate, const rb_stream_desc* descs,
                                size_t n_streams, uint32_t fifo_frames, uint32_t max_block_frames, uint32_t flags, rb_session** out);
@@ -388,6 +390,30 @@ rb_status rb_session_push(rb_session* s, size_t stream, const float* pcm, uint64
 /* The same for every source at once: pcm holds n_frames[0] frames of source 0, then n_frames[1] of source 1, ...;
  * end_of_stream may be NULL.  One host->device copy and one kernel for the whole session. */
 rb_status rb_session_push_packed(rb_session* s, const float* pcm, const uint64_t* n_frames, const uint8_t* end_of_stream);
+/* What current_span_len() starts to return during a push (RB_SESSION_RESTARTS): after `at` samples of THIS push have been
+ * pulled from the source it reports span_len (0 = None).  rodio's decoders report the length of the packet they decoded last
+ * (src/decoder/symphonia.rs:199-201), which changes as they play, and UniformSourceIterator asks at every bootstrap before it pulls
+ * (src/source/uniform.rs:50-68): a caller that pulls its source sample by sample records the report once before the first pull and
+ * after every pull, and passes the changes on as marks. */
+typedef struct rb_span_mark {
+    uint64_t at;        /* samples of this push the source has yielded when current_span_len() starts to return span_len */
+    uint32_t span_len;  /* 0 = None */
+    uint32_t pad_;      /* 0 */
+} rb_span_mark;
+/* rb_session_push / rb_session_push_packed with span marks.  desc.span_len is the report before the first mark; a mark holds until
+ * the next one, across pushes (a push without marks, by any of the push calls, leaves the report as it is).  Within a push `at`
+ * increases strictly and stays below n_frames * channels; a change seen after the last sample of a push goes at `at` = 0 of the
+ * next.  A bootstrap after the source has yielded p samples sees the last mark at or before p (the frames of
+ * rb_session_push_silence do not move p: the source is not pulled while paused); its run is min(report, 32768) samples, or less
+ * where a take ends first.  A block renders any number of restarts per source in one launch per class.  Sources at the mixer's
+ * rate take marks and ignore them.  RB_ERR_STATE: marks on a session created without RB_SESSION_RESTARTS;
+ * RB_ERR_INVALID_ARGUMENT: malformed marks; RB_ERR_UNSUPPORTED: a run would begin under a report that is not whole frames of the
+ * source or under two frames (also from rb_session_push_silence or a push without marks that reaches such a bootstrap).  A
+ * refused push changes nothing.  push_packed_spans: n_marks[i] marks for source i; `marks` holds those of source 0, then 1, ... */
+rb_status rb_session_push_spans(rb_session* s, size_t stream, const float* pcm, uint64_t n_frames, const rb_span_mark* marks,
+                                uint32_t n_marks, int end_of_stream);
+rb_status rb_session_push_packed_spans(rb_session* s, const float* pcm, const uint64_t* n_frames, const uint8_t* end_of_stream,
+                                       const uint32_t* n_marks, const rb_span_mark* marks);
 /* Player::pause / play for one source: n_frames frames of literal 0.0 behind its push program, what Pausable hands out while
  * paused (src/source/pausable.rs:85-97) -- the program in front is not pulled, so fades and takes stand still.  They take FIFO
  * room like a push (RB_ERR_BUFFER_TOO_SMALL).  RB_ERR_UNSUPPORTED for a source with a filter in front of the conversion:

@@ -391,6 +391,12 @@ class LiveMixer {
     void push(size_t i, const std::vector<Sample>& pcm, bool end_of_stream = false) {
         check(rb_session_push(h_, i, pcm.data(), pcm.size() / src_channels_.at(i), end_of_stream ? 1 : 0), "rb_session_push");
     }
+    // The same with span marks (restarts only): after marks[k].at samples of this push the source reports marks[k].span_len
+    // (0 = None) -- a decoder's packet lengths, as current_span_len() returns them (rb_session_push_spans).
+    void push(size_t i, const std::vector<Sample>& pcm, const std::vector<rb_span_mark>& marks, bool end_of_stream = false) {
+        check(rb_session_push_spans(h_, i, pcm.data(), pcm.size() / src_channels_.at(i), marks.data(), (uint32_t)marks.size(),
+                                    end_of_stream ? 1 : 0), "rb_session_push_spans");
+    }
     // Player::pause for n_frames frames: whole frames of 0.0 behind the source's push program, which is not pulled meanwhile
     void push_silence(size_t i, uint64_t n_frames) { check(rb_session_push_silence(h_, i, n_frames), "rb_session_push_silence"); }
     // Mixer::add (mixer.rs:58-66) for a source that was declared held (its desc().mix_start == RB_SESSION_HELD)

@@ -59,7 +59,12 @@ class rb_stream_desc(C.Structure):
     ]
 
 
+class rb_span_mark(C.Structure):
+    _fields_ = [("at", C.c_uint64), ("span_len", C.c_uint32), ("pad_", C.c_uint32)]
+
+
 assert C.sizeof(rb_effect) == 80
+assert C.sizeof(rb_span_mark) == 16
 
 # every symbol include/rodio_b200.h declares: (restype, argtypes)
 _u64p = C.POINTER(C.c_uint64)
@@ -107,6 +112,8 @@ SYMBOLS = {
     "rb_session_push": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint64, C.c_int]),
     "rb_session_push_packed": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rb_session_push_silence": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_uint64]),
+    "rb_session_push_spans": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint64, C.POINTER(rb_span_mark), C.c_uint32, C.c_int]),
+    "rb_session_push_packed_spans": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(rb_span_mark)]),
     "rb_session_start": (C.c_int32, [C.c_void_p, C.c_size_t]),
     "rb_session_follow": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_size_t]),
     "rb_session_skip": (C.c_int32, [C.c_void_p, C.c_size_t]),

@@ -1816,10 +1816,19 @@ struct rb_session {
     std::vector<uint8_t> no_silence;           // a take in front of a resampling conversion: rb_session_push_silence refused
     rb_prog_op* d_prog = nullptr;
     rb_fifo_prog_job *d_pjobs = nullptr, *h_pjobs = nullptr;
-    // restart schedules (RB_SESSION_RESTARTS, rb_session_plan.h): some source has one; the cuts of a block, per row
-    bool has_sched = false;
+    // restart schedules (RB_SESSION_RESTARTS, rb_session_plan.h): some source has one; the cuts of a block, rows in compressed
+    // sparse row form (cut_first: [rows + 1]), grown to the largest block's count
+    bool restarts = false, has_sched = false;
     lanes::Cut *d_cuts = nullptr, *h_cuts = nullptr;
+    uint32_t *d_cut_first = nullptr, *h_cut_first = nullptr;
+    size_t cut_cap = 0;
     uint64_t restart_launches = 0;             // launches of the lane kernel's RESTART twins so far
+    // span marks (rb_session_push_spans): per source, what current_span_len() reports at the pushed end (samples, 0: None) --
+    // desc.span_len until a mark says otherwise -- and the run cap a report of None gives (a take's, or none); `marked`: some push
+    // carried marks (the state blob is version 9 from then on)
+    std::vector<uint64_t> report, none_cap;
+    std::vector<uint8_t> follows_marks;        // the source is resampled in a session with RB_SESSION_RESTARTS: marks move its runs
+    bool marked = false;
 #if defined(RB_SIMT_EMULATE)
     std::vector<uint64_t> emu_fast_tiles;      // CPU build: fast tiles the emulator ran per class (rb_session_emu_fast_tiles)
 #endif
@@ -1833,7 +1842,7 @@ extern "C" rb_status rb_session_destroy(rb_session* s) {
     cudaFreeHost(s->h_rows), cudaFreeHost(s->h_u32), cudaFreeHost(s->h_jobs), cudaFreeHost(s->h_out);
     cudaFree(s->d_master[0]), cudaFree(s->d_master[1]), cudaFree(s->d_master_runs), cudaFreeHost(s->h_master_runs);
     cudaFree(s->d_prog), cudaFree(s->d_pjobs), cudaFreeHost(s->h_pjobs);
-    cudaFree(s->d_cuts), cudaFreeHost(s->h_cuts);
+    cudaFree(s->d_cuts), cudaFreeHost(s->h_cuts), cudaFree(s->d_cut_first), cudaFreeHost(s->h_cut_first);
     delete s;
     return RB_OK;
 }
@@ -1866,6 +1875,7 @@ extern "C" rb_status rb_session_create_ex(rb_context* ctx, uint16_t mixer_channe
     std::vector<uint64_t> take_n(n, ~0ull);   // samples the source's takes let through
     std::vector<uint8_t> no_silence(n, 0);
     std::vector<uint64_t> run_cap(n, 0);      // RB_SESSION_RESTARTS: frames per converter run (0: the source is one run)
+    std::vector<uint64_t> none_cap(n, session::NO_LIMIT);   // ... under a report of None
     for (size_t i = 0; i < n; i++) {
         const rb_stream_desc& d = descs[i];
         const std::string where = "stream " + std::to_string(i) + ": ";
@@ -1948,8 +1958,9 @@ extern "C" rb_status rb_session_create_ex(rb_context* ctx, uint16_t mixer_channe
             if (d.span_len % d.channels || (d.span_len > RB_UNIFORM_SPAN_CAP && !cap_whole))
                 return fail(RB_ERR_UNSUPPORTED, where + "restarts: span_len (capped at 32768 samples) must be whole frames of the source");
             take_runs = from[i] != to[i] && take_n[i] != ~0ull && take_n[i] % d.channels == 0 && (take_n[i] <= RB_UNIFORM_SPAN_CAP || cap_whole);
+            if (take_runs) none_cap[i] = cap_whole ? RB_UNIFORM_SPAN_CAP / d.channels : take_n[i] / d.channels;
             if (from[i] != to[i] && (d.span_len || take_runs)) {
-                run_cap[i] = d.span_len ? std::min(d.span_len, RB_UNIFORM_SPAN_CAP) / d.channels : cap_whole ? RB_UNIFORM_SPAN_CAP / d.channels : take_n[i] / d.channels;
+                run_cap[i] = d.span_len ? std::min(d.span_len, RB_UNIFORM_SPAN_CAP) / d.channels : none_cap[i];
                 if (run_cap[i] < 2) return fail(RB_ERR_UNSUPPORTED, where + "restarts: converter runs shorter than two frames");
             }
         }
@@ -1984,6 +1995,7 @@ extern "C" rb_status rb_session_create_ex(rb_context* ctx, uint16_t mixer_channe
     s->st.resize(n), s->coef.assign(5 * n, 0.0f), s->ffk.assign(n, 0.0f), s->post.assign(n, 1.0f), s->pre.assign(n, 1.0f), s->mid.assign(n, 1.0f), s->src_ch.assign(n, 1);
     s->vol_a.assign(n, 1.0f), s->vol_b.assign(n, 1.0f), s->pads.assign(n, 0);
     s->prog_op0.assign(n, 0), s->prog_n.assign(n, 0), s->prog_pos.assign(n, 0), s->prog_end.assign(n, ~0ull), s->no_silence.assign(n, 0);
+    s->restarts = restarts, s->report.assign(n, 0), s->none_cap.assign(n, session::NO_LIMIT), s->follows_marks.assign(n, 0);
     bool any_biquad = false;
     std::vector<uint8_t> row_ff2(n, 1);
     for (size_t r = 0; r < n; r++) {
@@ -2032,6 +2044,7 @@ extern "C" rb_status rb_session_create_ex(rb_context* ctx, uint16_t mixer_channe
         }
         s->st[r].mix_start = d.mix_start, s->st[r].from = from[i], s->st[r].to = to[i];
         s->st[r].run_cap = run_cap[i], s->has_sched = s->has_sched || run_cap[i] != 0;
+        s->report[r] = d.span_len, s->none_cap[r] = none_cap[i], s->follows_marks[r] = restarts && from[i] != to[i];
         if (d.mix_start == RB_SESSION_HELD) s->st[r].held = true, s->st[r].mix_start = 0;   // Mixer::add comes later (rb_session_start)
         s->src_ch[r] = (uint8_t)d.channels;
         s->max_src_ch = std::max<uint32_t>(s->max_src_ch, d.channels);
@@ -2108,10 +2121,6 @@ extern "C" rb_status rb_session_create_ex(rb_context* ctx, uint16_t mixer_channe
     RB_CUDA(cudaMallocHost(&s->h_u32, 2 * nr * sizeof(uint32_t)));
     RB_CUDA(cudaMallocHost(&s->h_jobs, nr * sizeof(rb_fifo_job)));
     RB_CUDA(cudaMallocHost(&s->h_out, pstride * sizeof(float)));
-    if (s->has_sched) {
-        RB_CUDA(cudaMalloc(&s->d_cuts, nr * sizeof(lanes::Cut)));
-        RB_CUDA(cudaMallocHost(&s->h_cuts, nr * sizeof(lanes::Cut)));
-    }
     RB_CUDA(cudaMemsetAsync(s->d_fifo[0], 0, arena, ctx->stream));
     RB_CUDA(cudaMemsetAsync(s->d_fifo[1], 0, arena, ctx->stream));
     RB_CUDA(cudaMemsetAsync(s->d_state, 0, nr * 8 * sizeof(float), ctx->stream));
@@ -2160,22 +2169,65 @@ static bool session_take_ended(const rb_session* s, size_t r) { return s->prog_p
 static uint64_t session_take_room(const rb_session* s, size_t r, uint64_t n) {
     return std::min(n, s->prog_end[r] - std::min(s->prog_end[r], s->prog_pos[r]));
 }
-// After `frames` frames went into source r: its program index advances; the take's last frame ends the source.
-static void session_pushed(rb_session* s, size_t r, uint64_t frames) {
-    session::schedule_push(s->st[r], frames, s->prog_end[r] == ~0ull ? ~0ull : s->prog_end[r] - std::min(s->prog_end[r], s->prog_pos[r]), true);
+// The frames the source's take still lets through (~0: no take).
+static uint64_t session_take_left(const rb_session* s, size_t r) {
+    return s->prog_end[r] == ~0ull ? ~0ull : s->prog_end[r] - std::min(s->prog_end[r], s->prog_pos[r]);
+}
+// After `frames` frames went into source r: its program index advances; the take's last frame ends the source.  `changes`: what
+// the push's span marks do to its runs (session_span_changes; checked by session_runs_ok beforehand).
+static void session_pushed(rb_session* s, size_t r, uint64_t frames, const std::vector<session::CapChange>& changes = {}) {
+    session::schedule_push(s->st[r], frames, session_take_left(s, r), true, changes.data(), changes.size());
+    s->has_sched = s->has_sched || s->st[r].run_cap != 0;
     s->st[r].pushed += frames;
     s->prog_pos[r] += frames;
     if (session_take_ended(s, r)) s->st[r].eof = true;
 }
-
-extern "C" rb_status rb_session_push(rb_session* s, size_t stream, const float* pcm, uint64_t n_frames, int end_of_stream) {
+// The run cap (frames) a report of `span_len` samples gives source r (source order): min(span_len, 32768) samples
+// (src/source/uniform.rs:55), BAD_CAP when that is not whole frames or under two; for None the take's cap, or none.
+static uint64_t session_report_cap(const rb_session* s, size_t r, uint64_t span_len) {
+    if (!span_len) return s->none_cap[r];
+    const uint64_t ch = s->src_ch[r], len = std::min<uint64_t>(span_len, RB_UNIFORM_SPAN_CAP);
+    return len % ch || len / ch < 2 ? session::BAD_CAP : len / ch;
+}
+// The span marks of one push into source r (source order) of n_frames frames: validated, and turned into the run caps they give
+// from the frame of the push at which a bootstrap first sees them (a mark at sample `at` counts for a bootstrap after at samples or
+// more).  A source that does not follow marks keeps only the report.  A run under a report must be whole frames and two of them at
+// least; that is checked where a run begins (session_runs_ok), so a report no bootstrap sees is never refused.
+static rb_status session_span_changes(const rb_session* s, size_t r, uint64_t n_frames, const rb_span_mark* marks, uint32_t n_marks,
+                                      std::vector<session::CapChange>* out) {
+    out->clear();
+    if (!n_marks) return RB_OK;
+    if (!s->restarts) return fail(RB_ERR_STATE, "span marks: the session was created without RB_SESSION_RESTARTS");
+    if (!marks) return fail(RB_ERR_INVALID_ARGUMENT, "span marks: marks is NULL");
+    const uint64_t ch = s->src_ch[r];
+    for (uint32_t k = 0; k < n_marks; k++) {
+        if (marks[k].pad_ != 0 || marks[k].at >= n_frames * ch || (k && marks[k].at <= marks[k - 1].at))
+            return fail(RB_ERR_INVALID_ARGUMENT, "span marks: `at` must increase strictly and stay inside the push, pad_ must be 0");
+        if (!s->follows_marks[r]) continue;
+        out->push_back(session::CapChange{(marks[k].at + ch - 1) / ch, session_report_cap(s, r, marks[k].span_len)});
+    }
+    return RB_OK;
+}
+// Would the runs a push of `frames` frames (real: PCM, else a pause's silence) begins into source r be served?
+static bool session_runs_ok(const rb_session* s, size_t r, uint64_t frames, bool real, const std::vector<session::CapChange>& changes = {}) {
+    if (!s->marked && changes.empty()) return true;   // without marks every run cap was checked when the session was created
+    session::Stream t = s->st[r];
+    return session::schedule_push(t, frames, session_take_left(s, r), real, changes.data(), changes.size());
+}
+static rb_status session_push_one(rb_session* s, size_t stream, const float* pcm, uint64_t n_frames, const rb_span_mark* marks,
+                                  uint32_t n_marks, int end_of_stream) {
     if (!s || (!pcm && n_frames)) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
     if (stream >= s->st.size()) return fail(RB_ERR_INVALID_ARGUMENT, "stream index out of range");
     stream = s->pos[stream];   // class order from here on
     session::Stream& st = s->st[stream];
+    std::vector<session::CapChange> changes;
+    rb_status rc = session_span_changes(s, stream, n_frames, marks, n_marks, &changes);
+    if (rc != RB_OK) return rc;
     if (st.eof) return n_frames && !session_take_ended(s, stream) ? fail(RB_ERR_STATE, "push after end_of_stream") : RB_OK;
     const uint64_t take = session_take_room(s, stream, n_frames);
     if (take > s->fifo_cap - st.fill()) return fail(RB_ERR_BUFFER_TOO_SMALL, "the stream's FIFO is full: render first");
+    if (!session_runs_ok(s, stream, take, true, changes))
+        return fail(RB_ERR_UNSUPPORTED, "span marks: a converter run would begin that is not whole frames of the source, or shorter than two");
     RB_CUDA(cudaSetDevice(s->ctx->device));
     if (take) {
         // one stream: into the staging buffer, scattered over the FIFOs of its rows
@@ -2184,10 +2236,20 @@ extern "C" rb_status rb_session_push(rb_session* s, size_t stream, const float* 
         RB_CUDA(cudaMemcpyAsync(s->d_stage, pcm, take * s->src_ch[stream] * sizeof(float), cudaMemcpyHostToDevice, stq));
         RB_CUDA(session_scatter(s, session_jobs(s, stream, 0, take, 0), stq));
         RB_CUDA(cudaStreamSynchronize(stq));   // the caller may reuse `pcm` as soon as we return
-        session_pushed(s, stream, take);
+        session_pushed(s, stream, take, changes);
     }
+    if (n_marks) s->report[stream] = marks[n_marks - 1].span_len, s->marked = true;
     if (end_of_stream) st.eof = true;
     return RB_OK;
+}
+
+extern "C" rb_status rb_session_push(rb_session* s, size_t stream, const float* pcm, uint64_t n_frames, int end_of_stream) {
+    return session_push_one(s, stream, pcm, n_frames, nullptr, 0, end_of_stream);
+}
+
+extern "C" rb_status rb_session_push_spans(rb_session* s, size_t stream, const float* pcm, uint64_t n_frames, const rb_span_mark* marks,
+                                           uint32_t n_marks, int end_of_stream) {
+    return session_push_one(s, stream, pcm, n_frames, marks, n_marks, end_of_stream);
 }
 
 extern "C" rb_status rb_session_push_silence(rb_session* s, size_t stream, uint64_t n_frames) {
@@ -2202,6 +2264,8 @@ extern "C" rb_status rb_session_push_silence(rb_session* s, size_t stream, uint6
     if (st.eof) return n_frames && !session_take_ended(s, r) ? fail(RB_ERR_STATE, "silence after end_of_stream") : RB_OK;
     if (n_frames > s->fifo_cap - st.fill()) return fail(RB_ERR_BUFFER_TOO_SMALL, "the stream's FIFO is full: render first");
     if (n_frames == 0) return RB_OK;
+    if (!session_runs_ok(s, r, n_frames, false))
+        return fail(RB_ERR_UNSUPPORTED, "silence: a converter run would begin under a span report that is not whole frames, or under two");
     RB_CUDA(cudaSetDevice(s->ctx->device));
     cudaStream_t stq = s->ctx->stream;
     for (uint32_t q : s->rows_of[r]) {   // literal +0.0 behind the program: inside the exact-reciprocal class, no flag to set
@@ -2209,21 +2273,30 @@ extern "C" rb_status rb_session_push_silence(rb_session* s, size_t stream, uint6
         RB_CUDA(cudaMemsetAsync(s->d_fifo[s->cur] + q * s->stride + st.fill() * ci, 0, n_frames * ci * sizeof(float), stq));
     }
     RB_CUDA(cudaStreamSynchronize(stq));
-    session::schedule_push(st, n_frames, s->prog_end[r] == ~0ull ? ~0ull : s->prog_end[r] - std::min(s->prog_end[r], s->prog_pos[r]), false);
+    session::schedule_push(st, n_frames, session_take_left(s, r), false);
     st.pushed += n_frames;   // the program's index stands still
     return RB_OK;
 }
 
-extern "C" rb_status rb_session_push_packed(rb_session* s, const float* pcm, const uint64_t* n_frames, const uint8_t* end_of_stream) {
+static rb_status session_push_many(rb_session* s, const float* pcm, const uint64_t* n_frames, const uint8_t* end_of_stream, const uint32_t* n_marks,
+                                   const rb_span_mark* marks) {
     if (!s || !n_frames) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
     const size_t ns = s->st.size();
     uint64_t total = 0;
     std::vector<uint64_t> take(ns);   // per caller's index: the frames the source's take lets through
-    for (size_t i = 0; i < ns; i++) {   // i: the caller's index, pos[i]: class order
+    std::vector<std::vector<session::CapChange>> changes(n_marks ? ns : 0);
+    for (size_t i = 0, m = 0; i < ns; i++) {   // i: the caller's index, pos[i]: class order
         const session::Stream& st = s->st[s->pos[i]];
+        if (n_marks) {
+            rb_status rc = session_span_changes(s, s->pos[i], n_frames[i], marks ? marks + m : nullptr, n_marks[i], &changes[i]);
+            if (rc != RB_OK) return fail(rc, "stream " + std::to_string(i) + ": " + rb_last_error());
+            m += n_marks[i];
+        }
         if (st.eof && n_frames[i] && !session_take_ended(s, s->pos[i])) return fail(RB_ERR_STATE, "stream " + std::to_string(i) + ": push after end_of_stream");
         take[i] = st.eof ? 0 : session_take_room(s, s->pos[i], n_frames[i]);
         if (take[i] > s->fifo_cap - st.fill()) return fail(RB_ERR_BUFFER_TOO_SMALL, "stream " + std::to_string(i) + ": FIFO full, render first");
+        if (!session_runs_ok(s, s->pos[i], take[i], true, n_marks ? changes[i] : std::vector<session::CapChange>{}))
+            return fail(RB_ERR_UNSUPPORTED, "stream " + std::to_string(i) + ": span marks: a converter run would begin that is not whole frames of the source, or shorter than two");
         total += n_frames[i];
     }
     if (total && !pcm) return fail(RB_ERR_INVALID_ARGUMENT, "pcm is NULL");
@@ -2249,11 +2322,27 @@ extern "C" rb_status rb_session_push_packed(rb_session* s, const float* pcm, con
         RB_CUDA(session_scatter(s, n_jobs, stq));
         RB_CUDA(cudaStreamSynchronize(stq));
     }
-    for (size_t i = 0; i < ns; i++) {
-        session_pushed(s, s->pos[i], take[i]);
+    for (size_t i = 0, m = 0; i < ns; i++) {
+        if (n_marks) {
+            session_pushed(s, s->pos[i], take[i], changes[i]);
+            if (n_marks[i]) s->report[s->pos[i]] = marks[m + n_marks[i] - 1].span_len, s->marked = true;
+            m += n_marks[i];
+        } else {
+            session_pushed(s, s->pos[i], take[i]);
+        }
         if (end_of_stream && end_of_stream[i]) s->st[s->pos[i]].eof = true;
     }
     return RB_OK;
+}
+
+extern "C" rb_status rb_session_push_packed(rb_session* s, const float* pcm, const uint64_t* n_frames, const uint8_t* end_of_stream) {
+    return session_push_many(s, pcm, n_frames, end_of_stream, nullptr, nullptr);
+}
+
+extern "C" rb_status rb_session_push_packed_spans(rb_session* s, const float* pcm, const uint64_t* n_frames, const uint8_t* end_of_stream,
+                                                  const uint32_t* n_marks, const rb_span_mark* marks) {
+    if (s && !n_marks) return fail(RB_ERR_INVALID_ARGUMENT, "n_marks is NULL");
+    return session_push_many(s, pcm, n_frames, end_of_stream, n_marks, marks);
 }
 
 extern "C" rb_status rb_session_start(rb_session* s, size_t stream) {
@@ -2351,19 +2440,11 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
     if (ended) *ended = e ? 1 : 0;
     if (n == 0) return RB_OK;
     if (!out_host) return fail(RB_ERR_INVALID_ARGUMENT, "out_host is NULL");
-    // The lane kernel walks one restart per row and launch: a block in which some source restarts twice (spans of a few frames)
-    // is rendered as sub-blocks that end where such a source's second run does.
-    while (*written < n) {
-        uint64_t k = n - *written;
-        if (s->has_sched)
-            for (session::Stream& st : s->st) {
-                session::settle(st);
-                if (!st.held && !session::finished(st)) k = std::min(k, session::one_cut_limit(st) - std::min(session::one_cut_limit(st), s->T));
-            }
-        rb_status rc = session_render_block(s, out_host + *written * s->channels, k);
-        if (rc != RB_OK) return rc;
-        *written += k;
-    }
+    if (s->has_sched)
+        for (session::Stream& st : s->st) session::settle(st);
+    rb_status rc = session_render_block(s, out_host, n);
+    if (rc != RB_OK) return rc;
+    *written = n;
     if (ended) {
         bool e2 = false;
         session::renderable(s->st, s->T, 1, &e2);
@@ -2372,7 +2453,25 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
     return RB_OK;
 }
 
-// One launch per class over the frames [T, T + n), which every source can supply and in which none restarts twice.
+// Room for n_cuts cuts of a block (and the row offsets of the cut lists): grown, never shrunk.
+static cudaError_t session_cut_buffers(rb_session* s, size_t n_cuts) {
+    cudaError_t e = cudaSuccess;
+    if (!s->d_cut_first) {
+        const size_t nr = s->rows.size();
+        if ((e = cudaMalloc(&s->d_cut_first, (nr + 1) * sizeof(uint32_t))) != cudaSuccess) return e;
+        if ((e = cudaMallocHost(&s->h_cut_first, (nr + 1) * sizeof(uint32_t))) != cudaSuccess) return e;
+    }
+    if (n_cuts <= s->cut_cap) return e;
+    const size_t cap = std::max(n_cuts, 2 * s->cut_cap);
+    cudaFree(s->d_cuts), cudaFreeHost(s->h_cuts);
+    s->d_cuts = nullptr, s->h_cuts = nullptr, s->cut_cap = 0;
+    if ((e = cudaMalloc(&s->d_cuts, cap * sizeof(lanes::Cut))) != cudaSuccess) return e;
+    if ((e = cudaMallocHost(&s->h_cuts, cap * sizeof(lanes::Cut))) != cudaSuccess) return e;
+    s->cut_cap = cap;
+    return e;
+}
+
+// One launch per class over the frames [T, T + n), which every source can supply; a source may restart any number of times in it.
 static rb_status session_render_block(rb_session* s, float* out_host, uint64_t n) {
     RB_CUDA(cudaSetDevice(s->ctx->device));
     cudaStream_t stq = s->ctx->stream;
@@ -2386,8 +2485,14 @@ static rb_status session_render_block(rb_session* s, float* out_host, uint64_t n
         if (!s->st[r].front && !(lanes::pre_gain_keeps_class(s->pre[r]) && lanes::pre_gain_keeps_class(s->vol_a[r]) && lanes::pre_gain_keeps_class(s->vol_b[r])))
             quiet[r] = 1;   // its class runs the guarded tile in this block (or, DOWN, slow tiles)
     }
-    bool any_cut = false;
-    for (size_t q = 0; q < nr; q++) {   // every row of a source renders the source's part: the rows stay in lock step
+    size_t n_cuts = 0;   // cuts of the block, over all rows
+    if (s->has_sched) {
+        for (size_t q = 0; q < nr; q++) n_cuts += parts[s->rows[q].src].cuts.size();
+        if (n_cuts > 0xFFFFFFFFull) return fail(RB_ERR_OUT_OF_MEMORY, "more than 2^32 converter restarts in one block");
+        RB_CUDA(session_cut_buffers(s, n_cuts));
+    }
+    const bool any_cut = n_cuts != 0;
+    for (size_t q = 0, k = 0; q < nr; q++) {   // every row of a source renders the source's part: the rows stay in lock step
         const size_t r = s->rows[q].src;
         const session::Part& p = parts[r];
         lanes::Row& row = s->h_rows[q];
@@ -2396,8 +2501,9 @@ static rb_status session_render_block(rb_session* s, float* out_host, uint64_t n
         row.in = fifo + q * s->stride, row.L = p.out_len ? p.run_end - s->st[r].i0 : s->st[r].fill(), row.out_len = p.out_len, row.mix_start = p.mix_start;
         row.n_int = p.n_int, row.o0 = p.o0, row.i0 = s->st[r].i0 - p.run_i, row.state = s->d_state + 8 * q;
         if (s->has_sched) {
-            s->h_cuts[q] = lanes::Cut{p.cut_m, p.cut_n_int, s->st[r].i0 - p.cut_i, p.cut_end - s->st[r].i0};
-            any_cut = any_cut || p.cut_m < p.out_len;
+            s->h_cut_first[q] = (uint32_t)k;
+            for (const session::RunCut& c : p.cuts) s->h_cuts[k++] = lanes::Cut{c.m, c.n_int, s->st[r].i0 - c.i, c.end - s->st[r].i0};
+            s->h_cut_first[q + 1] = (uint32_t)k;
         }
         const float* co = &s->coef[5 * r];
         row.b0 = co[0], row.b1 = co[1], row.b2 = co[2], row.a1 = co[3], row.a2 = co[4], row.ffk = s->ffk[r];
@@ -2406,7 +2512,10 @@ static rb_status session_render_block(rb_session* s, float* out_host, uint64_t n
         row.f0 = s->st[r].fpos - s->st[r].i0, row.ga = s->vol_a[r], row.gb = s->vol_b[r];
     }
     RB_CUDA(cudaMemcpyAsync(s->d_rows, s->h_rows, nr * sizeof(lanes::Row), cudaMemcpyHostToDevice, stq));
-    if (any_cut) RB_CUDA(cudaMemcpyAsync(s->d_cuts, s->h_cuts, nr * sizeof(lanes::Cut), cudaMemcpyHostToDevice, stq));
+    if (any_cut) {
+        RB_CUDA(cudaMemcpyAsync(s->d_cuts, s->h_cuts, n_cuts * sizeof(lanes::Cut), cudaMemcpyHostToDevice, stq));
+        RB_CUDA(cudaMemcpyAsync(s->d_cut_first, s->h_cut_first, (nr + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stq));
+    }
     const uint64_t pstride = lanes::round_up_tile((uint64_t)s->max_block * C);
     // rows of the partial buffer are only written inside each warp's span: clear what this block may read
     RB_CUDA(cudaMemsetAsync(s->d_partial, 0, (size_t)s->n_groups * pstride * sizeof(float), stq));
@@ -2421,17 +2530,18 @@ static rb_status session_render_block(rb_session* s, float* out_host, uint64_t n
         bool guard = false, cut = false;   // cut: some row of the class restarts in this block -- the class takes the RESTART twin
         for (uint32_t q = c.first; q < c.first + c.count; q++) {
             guard = guard || quiet[s->rows[q].src];
-            cut = cut || (any_cut && s->h_cuts[q].m < s->h_rows[q].out_len);
+            cut = cut || (any_cut && s->h_cut_first[q + 1] > s->h_cut_first[q]);
         }
 #if defined(RB_SIMT_EMULATE)
         const uint64_t fast0 = simt::g_emu_count[0];
 #endif
         if (cut) {
-            a.cuts = s->d_cuts + c.first;
+            a.cuts = s->d_cuts, a.cut_first = s->d_cut_first + c.first;
 #if defined(RB_SIMT_EMULATE)
             session_host::g_restart_readable.clear();
-            for (const auto& b : {std::pair<const void*, size_t>{fifo, nr * s->stride * sizeof(float)}, {s->d_rows, nr * sizeof(lanes::Row)}, {s->d_cuts, nr * sizeof(lanes::Cut)},
-                                  {s->d_state, nr * 8 * sizeof(float)}, {s->d_zeros, 256}, {s->d_flags, nr * sizeof(uint32_t)}})
+            for (const auto& b : {std::pair<const void*, size_t>{fifo, nr * s->stride * sizeof(float)}, {s->d_rows, nr * sizeof(lanes::Row)}, {s->d_cuts, n_cuts * sizeof(lanes::Cut)},
+                                  {s->d_cut_first, (nr + 1) * sizeof(uint32_t)}, {s->d_state, nr * 8 * sizeof(float)}, {s->d_zeros, 256},
+                                  {s->d_flags, nr * sizeof(uint32_t)}})
                 session_host::g_restart_readable.push_back({(const char*)b.first, (const char*)b.first + b.second});
 #endif
             RB_CUDA(rb_lanes_launch_restart(a, c.ch_in, c.ch_out, c.has_biquad, c.front, stq));
@@ -2563,15 +2673,18 @@ struct SessionBlobProg {
 // Version 8 (a session some source of which has a restart schedule): version 6 or, with push programs, 7, then one run record per
 // source (source order), each followed by its n_ends run ends, then the FIFO contents.  A blob only restores a session with the
 // same schedules.
+// Version 9 (a session some push of which carried span marks): version 8 with the source's report at the pushed end (samples,
+// 0: None) behind each run record, in front of its run ends; the run cap is the one that report gives.  It restores into any
+// session of the same shape created with RB_SESSION_RESTARTS.
 struct SessionBlobRun {
     uint64_t run_cap, run_i, run_o, sched_end, runs_done, n_ends;
 };
 constexpr uint32_t SESSION_MAGIC = 0x52425353u;   // "RBSS"
-uint32_t blob_version(const rb_session* s) { return s->has_sched ? 8u : s->has_prog ? 7u : s->plain ? 5u : 6u; }
+uint32_t blob_version(const rb_session* s) { return s->marked ? 9u : s->has_sched ? 8u : s->has_prog ? 7u : s->plain ? 5u : 6u; }
 uint64_t blob_run_bytes(const rb_session* s) {
     uint64_t n = 0;
-    if (s->has_sched)
-        for (const session::Stream& st : s->st) n += sizeof(SessionBlobRun) + st.ends.size() * sizeof(uint64_t);
+    if (s->has_sched || s->marked)
+        for (const session::Stream& st : s->st) n += sizeof(SessionBlobRun) + (s->marked ? sizeof(uint64_t) : 0) + st.ends.size() * sizeof(uint64_t);
     return n;
 }
 SessionBlobSlot blob_slot(const rb_session::Slot& sl) { return {sl.src, (uint32_t)sl.ch0 | (uint32_t)sl.w << 8 | (uint32_t)sl.ci << 16}; }
@@ -2619,10 +2732,12 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
         }
         memcpy(p, s->prog_ops.data(), s->prog_ops.size() * sizeof(rb_prog_op)), p += s->prog_ops.size() * sizeof(rb_prog_op);
     }
-    if (s->has_sched)
-        for (const session::Stream& st : s->st) {
+    if (s->has_sched || s->marked)
+        for (size_t r = 0; r < ns; r++) {
+            const session::Stream& st = s->st[r];
             const SessionBlobRun b{st.run_cap, st.run_i, st.run_o, st.sched_end, st.runs_done, st.ends.size()};
             memcpy(p, &b, sizeof(b)), p += sizeof(b);
+            if (s->marked) memcpy(p, &s->report[r], sizeof(uint64_t)), p += sizeof(uint64_t);
             memcpy(p, st.ends.data(), st.ends.size() * sizeof(uint64_t)), p += st.ends.size() * sizeof(uint64_t);
         }
     for (size_t q = 0; q < nr; q++) {
@@ -2652,16 +2767,18 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
 extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64_t size) {
     if (!s || !buf) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
     const size_t nr = s->rows.size(), ns = s->st.size();
-    const uint64_t n_slots = blob_version(s) == 5u ? 0 : nr;
     const uint64_t prog_bytes = s->has_prog ? ns * sizeof(SessionBlobProg) + s->prog_ops.size() * sizeof(rb_prog_op) : 0;
     const uint8_t* p = (const uint8_t*)buf;
     SessionBlobHeader h;
     if (size < sizeof(h)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
     memcpy(&h, p, sizeof(h)), p += sizeof(h);
     const uint32_t C = s->channels;
-    if (h.magic != SESSION_MAGIC || h.version < 5u || h.version > 8u) return fail(RB_ERR_INVALID_ARGUMENT, "not a session state blob");
-    if (h.version != blob_version(s) || h.n_streams != nr || h.has_biquad != (s->has_biquad ? 1u : 0u) || h.channels != C)
+    if (h.magic != SESSION_MAGIC || h.version < 5u || h.version > 9u) return fail(RB_ERR_INVALID_ARGUMENT, "not a session state blob");
+    // a version-9 blob (span marks) restores into a session of the same shape with RB_SESSION_RESTARTS, marked or not
+    const bool v9 = h.version == 9u;
+    if ((v9 ? !s->restarts : h.version != blob_version(s)) || h.n_streams != nr || h.has_biquad != (s->has_biquad ? 1u : 0u) || h.channels != C)
         return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session of another shape");
+    const uint64_t n_slots = h.version == 5u ? 0 : nr;
     uint64_t need = sizeof(h) + nr * sizeof(SessionBlobStream) + n_slots * sizeof(SessionBlobSlot) + prog_bytes;
     if (size < need) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
     std::vector<SessionBlobStream> recs(nr);
@@ -2685,13 +2802,21 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
         p += s->prog_ops.size() * sizeof(rb_prog_op);
     }
     std::vector<session::Stream> runs(ns);   // the run records, checked against the source's record below
-    if (s->has_sched) {
+    std::vector<uint64_t> report = s->report;
+    if (h.version >= 8u) {
         const uint8_t* const end = (const uint8_t*)buf + size;
         for (size_t r = 0; r < ns; r++) {
             SessionBlobRun b;
             if ((uint64_t)(end - p) < sizeof(b)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
             memcpy(&b, p, sizeof(b)), p += sizeof(b);
-            if (b.run_cap != s->st[r].run_cap || (!b.run_cap && (b.n_ends || b.run_i || b.run_o)))
+            if (v9) {   // the run cap is the one the report gives, for a source that follows marks and has a schedule
+                if ((uint64_t)(end - p) < sizeof(uint64_t)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
+                memcpy(&report[r], p, sizeof(uint64_t)), p += sizeof(uint64_t), need += sizeof(uint64_t);
+                const bool eof = recs[s->rows_of[r][0]].eof != 0;   // (a take that has ended takes no more runs, nor their caps)
+                if (b.run_cap && s->follows_marks[r] && !eof && b.run_cap != session_report_cap(s, r, report[r]))
+                    return fail(RB_ERR_INVALID_ARGUMENT, "state blob: run cap and span report disagree");
+            }
+            if ((v9 ? !s->follows_marks[r] && b.run_cap : b.run_cap != s->st[r].run_cap) || (!b.run_cap && (b.n_ends || b.run_i || b.run_o)))
                 return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session with other restart schedules");
             if (b.n_ends > (uint64_t)(end - p) / sizeof(uint64_t)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
             session::Stream& st = runs[r];
@@ -2744,6 +2869,10 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
         st.mix_start = b.mix_start, st.pushed = b.pushed, st.out_done = b.out_done, st.i0 = b.i0, st.eof = b.eof != 0, st.fpos = b.i0 + b.filter_ahead, s->vol_a[r] = b.vol_a, s->vol_b[r] = b.vol_b;
         st.held = b.held != 0, st.follows = b.follows < 0 ? -1 : (int64_t)s->rows[(size_t)b.follows].src;
         st.run_i = runs[r].run_i, st.run_o = runs[r].run_o, st.sched_end = runs[r].sched_end, st.runs_done = runs[r].runs_done, st.ends = runs[r].ends;
+        if (v9) {   // the report is the state: the cap of the runs the next bootstraps begin follows from it
+            st.run_cap = runs[r].run_cap && s->follows_marks[r] && !st.eof ? session_report_cap(s, r, report[r]) : runs[r].run_cap;
+            s->has_sched = s->has_sched || st.run_cap != 0;
+        }
         (st.front ? s->mid[r] : s->pre[r]) = b.vol;
         if (b.post != s->post[r]) s->post[r] = b.post, s->has_post = true;
     }
@@ -2765,5 +2894,6 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
     RB_CUDA(cudaStreamSynchronize(s->ctx->stream));
     s->T = h.T;
     if (s->has_prog) s->prog_pos = prog_pos;
+    if (v9) s->report = report, s->marked = true;
     return RB_OK;
 }

@@ -380,7 +380,7 @@ static void launch_restart_cc(const lanes::Args& a, bool has_biquad, bool front,
 
 cudaError_t rb_lanes_launch_restart(const lanes::Args& a, uint32_t ch_in, uint32_t ch_out, bool has_biquad, bool front, cudaStream_t st) {
     if (a.mix_len == 0 || a.n_groups == 0) return cudaSuccess;
-    if (!a.cuts || a.from == a.to || (front && !has_biquad)) return cudaErrorInvalidValue;
+    if (!a.cuts || !a.cut_first || a.from == a.to || (front && !has_biquad)) return cudaErrorInvalidValue;
     if (!((ch_in == 1 || ch_in == 2) && (ch_in == ch_out || (ch_in == 1 && ch_out == 2)))) return cudaErrorInvalidValue;
     if (ch_in == 2) launch_restart_cc<2, 2>(a, has_biquad, front, st);
     else if (ch_out == 2) launch_restart_cc<1, 2>(a, has_biquad, front, st);

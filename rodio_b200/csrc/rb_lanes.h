@@ -52,8 +52,8 @@ void rb_lanes_destroy(rb_lanes_plan* p);
 // per stream, ch_out channels in the mixer) ...
 cudaError_t rb_lanes_launch_kernel(const lanes::Args& a, uint32_t ch_in, uint32_t ch_out, bool has_biquad, bool ff2, bool has_post,
                                    bool has_pre, bool front, bool guard, cudaStream_t st);
-// The same launch for a class some row of which changes its converter run inside the block (a.cuts, rb_lanes_core.h: Cut; never a
-// same-rate class).  Rows, groups and the bits of rows without a cut are those of rb_lanes_launch_kernel.
+// The same launch for a class some row of which changes its converter run inside the block, any number of times (a.cuts and
+// a.cut_first, rb_lanes_core.h: Cut; never a same-rate class).  Rows, groups and the bits of rows without a cut are those of rb_lanes_launch_kernel.
 cudaError_t rb_lanes_launch_restart(const lanes::Args& a, uint32_t ch_in, uint32_t ch_out, bool has_biquad, bool front, cudaStream_t st);
 // k_fused_duo (rb_duo_core.h) over a.rows: mono sources below the mixer's rate, two rows per lane, a.n_groups groups of 64
 cudaError_t rb_duo_launch_kernel(const lanes::Args& a, bool has_biquad, bool ff2, bool has_post, cudaStream_t st);

@@ -113,13 +113,14 @@ struct Row {                 // one stream (whole, or the part of it one block o
                              // a frame keeps the factor it was multiplied with when Amplify::next pulled it)
 };
 
-// RESTART (streaming sessions): the converter run of the row ends inside the block and the next one begins -- rodio's
+// RESTART (streaming sessions): converter runs of the row end inside the block and the next ones begin -- rodio's
 // UniformSourceIterator bootstraps a fresh SampleRateConverter there (src/source/uniform.rs:83-96), which interpolates inside
-// itself only, emits its last frame raw and starts again at numerator 0 with two new frames.  The Row describes the run that
-// ends (L, n_int, o0, i0 up to its last frame); from block-local output m on the lane walks the new run.  Filter state and gains
-// pass through; a filter in FRONT consumes every input frame once, in order, across the cut.
+// itself only, emits its last frame raw and starts again at numerator 0 with two new frames.  The Row describes the run of the
+// block's first output (L, n_int, o0, i0 up to its last frame); a row has any number of cuts, in timeline order, and from the
+// block-local output m of each the lane walks that cut's run.  Filter state and gains pass through; a filter in FRONT consumes
+// every input frame once, in order, across every cut.
 struct Cut {
-    uint64_t m;              // first output of the new run, relative to Row::mix_start; >= Row::out_len: no cut in this block
+    uint64_t m;              // first output of the new run, relative to Row::mix_start (< Row::out_len, increasing along a row)
     uint64_t n_int;          // of the outputs [m, out_len) the first n_int interpolate
     uint64_t i0;             // Row::i0 of the new run, whose o0 is 0: its first frame is in[-i0] (modulo 2^64)
     uint64_t L;              // Row::L of the new run
@@ -147,7 +148,8 @@ struct Args {
     const float* zeros;      // CHUNK zeros, 16-byte aligned: the source of idle lanes
     const uint32_t* unsafe;  // optional [n_rows]: non-zero = as if ROW_UNSAFE were set (streaming: kept on the device)
     const GroupSpan* spans;  // optional [n_groups] (rb_duo_core.h)
-    const Cut* cuts;         // RESTART: [n_rows]
+    const Cut* cuts;         // RESTART: the cuts of row r are cuts[cut_first[r] .. cut_first[r + 1]) (compressed sparse rows)
+    const uint32_t* cut_first;   // RESTART: [n_rows + 1]
 };
 
 // (t - a1*y1) - a2*y2, each product and each difference rounded once (src/source/blt.rs:558-560)
@@ -192,9 +194,9 @@ SIMT_FN float reduce_tile(const float (&v)[TILE], uint32_t ln) {
 // applied (no PRE twin).  Larger ratios stay on the slow tiles.  With FRONT the one or two frames an output moves on are
 // one or two steps of the filter.
 //
-// RESTART: rows may change their converter run once inside the block (Cut above).  The tile that holds a lane's cut is a slow
-// tile -- the ending run's fast tiles stop where its interpolating outputs do -- whose closed form switches to the new run at
-// the cut; the fast run behind it is primed from the new run's (o0 = 0, i0).
+// RESTART: rows may change their converter run any number of times inside the block (Cut above).  A tile that holds a lane's cut
+// is a slow tile -- the ending run's fast tiles stop where its interpolating outputs do -- whose closed form switches to the new
+// run at the cut; a fast run between two cuts is primed from the new run's (o0 = 0, i0).
 //
 // GUARD (with PRE): some stream of the class has a gain in front outside [2^-6, 2^6] (a Player at -40 dB): its scaled taps may
 // leave the range in which the reciprocal division is exact, so the tile checks every quotient like FRONT does and the
@@ -258,19 +260,23 @@ SIMT_FN void warp_main(const Args& a, uint32_t group, float* ring_warp) {
     // stream-absolute numerator of local output frame o is (o0 + o) * from; the input frame it falls on, relative to
     // in[0], is that / to - i0.  Both offsets are zero for whole streams.
     uint64_t o0 = row.o0, i0 = row.i0;
-    // RESTART: the lane walks the ending run up to timeline frame cut_t and moves to the new one when it gets there
-    Cut cut;
+    // RESTART: the lane walks its current run up to timeline frame cut_t (the next cut) and moves to that cut's run when it gets
+    // there; the last run ends with the row
+    uint32_t ck = 0;
     uint64_t cut_t = ~0ull;
-    if (RESTART && has && a.cuts[r].m < row.out_len) {
-        cut = a.cuts[r];
-        cut_t = ms + cut.m;
-        end = cut_t, stops = false;
+    if (RESTART && has) {
+        ck = a.cut_first[r];
+        if (ck < a.cut_first[r + 1]) cut_t = ms + a.cuts[ck].m, end = cut_t, stops = false;
     }
     auto restart_at = [&](uint64_t tt) {
-        if (RESTART && tt >= cut_t) {
-            ms = cut_t, end = row.mix_start + row.out_len, stops = !(row.flags & ROW_CONTINUES);
-            o0 = 0, i0 = cut.i0, L = cut.L, n_int = cut.n_int;
-            cut_t = ~0ull;
+        if (RESTART && tt >= cut_t) {   // (every run has an output: one cut per frame at most)
+            const Cut cut = a.cuts[ck++];
+            ms = cut_t, o0 = 0, i0 = cut.i0, L = cut.L, n_int = cut.n_int;
+            if (ck < a.cut_first[r + 1]) {
+                cut_t = row.mix_start + a.cuts[ck].m, end = cut_t;
+            } else {
+                cut_t = ~0ull, end = row.mix_start + row.out_len, stops = !(row.flags & ROW_CONTINUES);
+            }
         }
     };
     const uint32_t cq = ln % QPC;                      // the quad of a chunk this lane copies ...

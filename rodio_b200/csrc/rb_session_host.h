@@ -31,7 +31,7 @@ void restart_cc(const lanes::Args& a, uint32_t g, simt::WarpEmu* w, float* ring,
 
 cudaError_t rb_lanes_launch_restart(const lanes::Args& a, uint32_t ch_in, uint32_t ch_out, bool has_biquad, bool front, cudaStream_t) {
     if (a.mix_len == 0 || a.n_groups == 0) return cudaSuccess;
-    if (!a.cuts || a.from == a.to || (front && !has_biquad)) return cudaErrorInvalidValue;
+    if (!a.cuts || !a.cut_first || a.from == a.to || (front && !has_biquad)) return cudaErrorInvalidValue;
     if (!((ch_in == 1 || ch_in == 2) && (ch_in == ch_out || (ch_in == 1 && ch_out == 2)))) return cudaErrorInvalidValue;
     simt::WarpEmu warp;
     warp.readable = session_host::g_restart_readable;

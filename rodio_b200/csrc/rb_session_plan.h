@@ -19,6 +19,9 @@
 //     (src/source/uniform.rs:50-68, :83-96); the run pulls its first two frames at once, interpolates inside itself only and emits
 //     its last frame raw.  A stream with a schedule keeps the run the next output belongs to -- its first input and output frame --
 //     and the ends of the runs the pushes have begun; everything above applies to each run with indices relative to its start.
+//     What the source reports may change as it plays (a decoder reports the length of the packet it decoded last,
+//     src/decoder/symphonia.rs:199-201): the pushes carry those changes, and every bootstrap a push begins takes the report in
+//     effect at its position.  A run's end is fixed when it begins, so the only state is the report at the pushed end.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -42,7 +45,9 @@ struct Stream {
     bool front = false;        // the source's filter sits in front of the conversion, runs once per INPUT frame and has
                                // consumed exactly those frames: the FIFO must keep everything from fpos on
     // ---- restart schedule; run_cap == 0: none, the source is one run (every session without RB_SESSION_RESTARTS) ----
-    uint64_t run_cap = 0;      // frames a run holds at most: min(span_len, 32768) samples
+    uint64_t run_cap = 0;      // frames a run that begins now holds at most, from the report in effect at the pushed end:
+                               // min(report, 32768) samples; NO_LIMIT: None (the run lasts as long as the source); BAD_CAP: a
+                               // report no run may begin under (not whole frames, or under two)
     uint64_t run_i = 0;        // the run of output `out_done`: its first input frame ...
     uint64_t run_o = 0;        // ... and its first output frame (stream-absolute)
     uint64_t sched_end = 0;    // input frame at which the run the pushes are filling ends (0: nothing pushed yet)
@@ -63,18 +68,47 @@ inline uint64_t out_total(uint64_t L, uint32_t from, uint32_t to) {
 inline uint64_t out_interp(uint64_t L, uint32_t from, uint32_t to) {
     return L < 2 ? 0 : ((L - 1) * (uint64_t)to + from - 1) / from;
 }
+constexpr uint64_t NO_LIMIT = ~0ull;       // run_cap: the source reports None (and no take limits it)
+constexpr uint64_t BAD_CAP = ~0ull - 1;    // run_cap: a run may not begin under the report in effect
+// A change of what the source reports, inside a push: bootstraps from frame `at` of the push on begin runs of at most `cap` frames.
+struct CapChange {
+    uint64_t at, cap;
+};
 // A push of n frames (PCM, or a pause's silence: real = false) is about to move `pushed`: the runs whose first frame is among
 // them begin.  A run's length is known when it begins -- run_cap, or what the source's take still lets through at that moment
 // (take_left frames, ~0: no take; src/source/take.rs:180-196), the silence inside the run counted against it as rodio's Take
-// counts Pausable's zeros.
-inline void schedule_push(Stream& s, uint64_t n, uint64_t take_left, bool real) {
-    if (!s.run_cap) return;
+// counts Pausable's zeros.  changes[0 .. n_changes) (increasing `at`) move run_cap as the push goes: a bootstrap at frame k of the
+// push sees those with at <= k; run_cap ends as the push leaves it.  A stream without a schedule only takes one when its first
+// bootstrap -- frame 0 of its first push -- sees a limit.  Returns false, having changed nothing, when a run would begin under
+// BAD_CAP.
+inline bool schedule_push(Stream& s, uint64_t n, uint64_t take_left, bool real, const CapChange* changes = nullptr, size_t n_changes = 0) {
+    size_t c = 0;
+    auto apply = [&](uint64_t k) {
+        for (; c < n_changes && changes[c].at <= k; c++) s.run_cap = changes[c].cap;
+    };
+    if (!s.run_cap) {
+        if (s.pushed || !n_changes || changes[0].at || n == 0) return true;
+        const Stream keep = s;
+        apply(0);
+        if (s.run_cap == NO_LIMIT) s.run_cap = 0;   // None at the first bootstrap: one run for good
+        if (!s.run_cap) return true;
+        if (!schedule_push(s, n, take_left, real, changes + c, n_changes - c)) return s = keep, false;
+        return true;
+    }
+    const Stream keep = s;
     for (uint64_t at = s.pushed, stop = s.pushed + n; at < stop;) {
-        if (at == s.sched_end) s.sched_end = at + std::min(s.run_cap, take_left), s.ends.push_back(s.sched_end);
+        if (at == s.sched_end) {
+            apply(at - s.pushed);
+            if (s.run_cap == BAD_CAP) return s = keep, false;
+            const uint64_t len = std::min(s.run_cap, take_left);
+            s.sched_end = len >= NO_LIMIT - at ? NO_LIMIT : at + len, s.ends.push_back(s.sched_end);
+        }
         const uint64_t step = std::min(stop, s.sched_end) - at;
         if (real && take_left != ~0ull) take_left -= step;
         at += step;
     }
+    apply(NO_LIMIT);
+    return true;
 }
 // Output frames of stream `s` that exist so far (renderable): everything once it has ended, else the interpolated ones.  With a
 // schedule, run by run: a run whose last frame has arrived is complete, its raw last frame included, whatever follows.
@@ -102,11 +136,6 @@ inline void settle(Stream& s) {
 }
 // Converter runs that have produced an output so far.
 inline uint64_t runs_started(const Stream& s) { return s.runs_done + (s.out_done > s.run_o ? 1 : 0); }
-// A block renders at most one restart per stream: the timeline frame up to which a block may go (after settle).
-inline uint64_t one_cut_limit(const Stream& s) {
-    if (s.ends.size() < 3) return ~0ull;
-    return s.mix_start + s.run_o + out_total(s.ends[0] - s.run_i, s.from, s.to) + out_total(s.ends[1] - s.ends[0], s.from, s.to);
-}
 
 // How many mixer frames [T, T + n) can be rendered now (every unfinished stream must be able to supply its part).
 // Returns 0 with *ended = true when no stream is left (MixerSource::next returns None, src/mixer.rs:129-135).
@@ -145,21 +174,24 @@ inline uint64_t renderable(const std::vector<Stream>& st, uint64_t T, uint64_t m
     return active ? n : 0;        // nothing is playing: MixerSource::next() is None, the timeline stands still (mixer.rs:129-135)
 }
 
+// A restart inside a block: outputs from block-local m on belong to the run that begins at input frame i, has frames up to `end`
+// so far and interpolates on its first n_int outputs (of those in the block)
+struct RunCut {
+    uint64_t m, i, end, n_int;
+};
 // One stream's part of the block [T, T + n).
 struct Part {
     uint64_t mix_start = 0;   // block-local timeline position of its first output
     uint64_t out_len = 0;     // outputs it contributes
     uint64_t o0 = 0;          // index of the first of them in its converter run (stream-absolute without a schedule)
-    uint64_t n_int = 0;       // how many of them interpolate (the rest is the raw last frame); with a cut: of those in front of it
+    uint64_t n_int = 0;       // how many of them interpolate (the rest is the raw last frame); with cuts: of those in front of the first
     bool continues = false;   // more outputs will follow in later blocks
     uint64_t o_abs = 0;       // stream-absolute index of the first output
     uint64_t run_i = 0;       // first input frame of the run of o0 (stream-absolute) ...
     uint64_t run_end = 0;     // ... and the frame behind the last one of it that has arrived
-    // the block's restart: outputs [cut_m, out_len) belong to the next run (cut_m == out_len: none), which begins at input frame
-    // cut_i, has frames up to cut_end so far and interpolates on its first cut_n_int outputs
-    uint64_t cut_m = 0, cut_i = 0, cut_end = 0, cut_n_int = 0;
+    std::vector<RunCut> cuts;  // the block's restarts, in order: any number of runs may begin inside it
 };
-// (after settle; a block stays within one_cut_limit of every stream)
+// (after settle)
 inline Part part_of(const Stream& s, uint64_t T, uint64_t n) {
     Part p;
     if (s.held) {
@@ -173,17 +205,18 @@ inline Part part_of(const Stream& s, uint64_t T, uint64_t n) {
         p.continues = !finished(s);
         return p;
     }
-    p.mix_start = lo - T, p.out_len = p.cut_m = hi - lo, p.o_abs = lo - s.mix_start;
+    p.mix_start = lo - T, p.out_len = hi - lo, p.o_abs = lo - s.mix_start;
     p.run_i = s.run_i, p.run_end = s.run_cap ? std::min(s.pushed, s.ends[0]) : s.pushed;
     p.o0 = p.o_abs - s.run_o;
     const uint64_t ni = out_interp(p.run_end - p.run_i, from, to);
     p.n_int = ni > p.o0 ? std::min(p.out_len, ni - p.o0) : 0;
     p.continues = !(s.eof && p.o_abs + p.out_len >= ready);
-    if (s.run_cap && s.ends.size() > 1) {   // the current run is complete: does the block go past its last output?
-        const uint64_t run_out = out_total(p.run_end - p.run_i, from, to);
-        if (p.o0 + p.out_len > run_out) {
-            p.cut_m = run_out - p.o0, p.cut_i = s.ends[0], p.cut_end = std::min(s.pushed, s.ends[1]);
-            p.cut_n_int = std::min(p.out_len - p.cut_m, out_interp(p.cut_end - p.cut_i, from, to));
+    if (s.run_cap && s.ends.size() > 1) {   // the current run is complete: the runs behind it that the block reaches
+        uint64_t m = out_total(p.run_end - p.run_i, from, to) - p.o0;
+        for (size_t k = 1; k < s.ends.size() && m < p.out_len; k++) {
+            const uint64_t i = s.ends[k - 1], e = std::min(s.pushed, s.ends[k]);
+            p.cuts.push_back(RunCut{m, i, e, std::min(p.out_len - m, out_interp(e - i, from, to))});
+            m += out_total(e - i, from, to);
         }
     }
     return p;
@@ -208,9 +241,9 @@ inline void skip(Stream& s) {
 // After the block: advance the stream and tell how many FIFO frames (from the front) are dead.
 inline uint64_t advance(Stream& s, const Part& p) {
     if (p.out_len) {   // the converter (and a filter in front of it) stands behind the right neighbour of the block's last output
-        const bool cut = p.cut_m < p.out_len;   // ... in the run of that output: a new run pulls its first two frames at once
-        const uint64_t ia = ((cut ? p.out_len - 1 - p.cut_m : p.o0 + p.out_len - 1) * (uint64_t)s.from) / s.to;
-        s.fpos = std::min((cut ? p.cut_i : p.run_i) + ia + 2, cut ? p.cut_end : p.run_end);
+        const RunCut* c = p.cuts.empty() ? nullptr : &p.cuts.back();   // ... in the run of that output: a new run pulls its first
+        const uint64_t ia = ((c ? p.out_len - 1 - c->m : p.o0 + p.out_len - 1) * (uint64_t)s.from) / s.to;   // two frames at once
+        s.fpos = std::min((c ? c->i : p.run_i) + ia + 2, c ? c->end : p.run_end);
     }
     s.out_done = p.out_len ? p.o_abs + p.out_len : s.out_done;
     settle(s);

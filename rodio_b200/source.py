@@ -740,19 +740,34 @@ class Session:
     def __exit__(self, *a):
         self.close()
 
-    def push(self, stream: int, pcm, end_of_stream: bool = False):
+    def push(self, stream: int, pcm, end_of_stream: bool = False, spans: Optional[Sequence[Tuple[int, int]]] = None):
+        """spans: [(at, span_len), ...] -- after `at` samples of this push the source's current_span_len() is span_len (0: None),
+        for a session with restarts (rb_session_push_spans); None or empty: the report stays as it is."""
         a = np.ascontiguousarray(pcm, dtype=np.float32)
         ch = self.src_channels[stream]
         assert a.size % ch == 0, "whole frames"
+        if spans:
+            m = _span_marks(spans)
+            check(lib().rb_session_push_spans(self._h, stream, a.ctypes.data_as(C.c_void_p), a.size // ch, m, len(spans), int(end_of_stream)),
+                  "rb_session_push_spans")
+            return
         check(lib().rb_session_push(self._h, stream, a.ctypes.data_as(C.c_void_p), a.size // ch, int(end_of_stream)), "rb_session_push")
 
-    def push_packed(self, blocks: Sequence[np.ndarray], end_of_stream: Optional[Sequence[bool]] = None):
-        """One block per source (possibly empty), pushed with one copy and one kernel."""
+    def push_packed(self, blocks: Sequence[np.ndarray], end_of_stream: Optional[Sequence[bool]] = None,
+                    spans: Optional[Sequence[Sequence[Tuple[int, int]]]] = None):
+        """One block per source (possibly empty), pushed with one copy and one kernel.  spans: one list of (at, span_len) marks per
+        source, as in push (rb_session_push_packed_spans)."""
         assert len(blocks) == len(self.sources)
         blocks = [np.ascontiguousarray(b, dtype=np.float32) for b in blocks]
         flat = np.concatenate(blocks) if blocks else np.zeros(0, np.float32)
         n = (C.c_uint64 * len(blocks))(*[b.size // ch for b, ch in zip(blocks, self.src_channels)])
         eos = (C.c_uint8 * len(blocks))(*[int(bool(e)) for e in end_of_stream]) if end_of_stream is not None else None
+        if spans is not None:
+            assert len(spans) == len(self.sources)
+            counts = (C.c_uint32 * len(blocks))(*[len(m) for m in spans])
+            m = _span_marks([x for sp in spans for x in sp])
+            check(lib().rb_session_push_packed_spans(self._h, flat.ctypes.data_as(C.c_void_p), n, eos, counts, m), "rb_session_push_packed_spans")
+            return
         check(lib().rb_session_push_packed(self._h, flat.ctypes.data_as(C.c_void_p), n, eos), "rb_session_push_packed")
 
     def push_silence(self, stream: int, n_frames: int):
@@ -817,6 +832,13 @@ class Session:
     def set_state(self, blob: bytes):
         buf = (C.c_uint8 * len(blob)).from_buffer_copy(blob)
         check(lib().rb_session_set_state(self._h, buf, len(blob)), "rb_session_set_state")
+
+
+def _span_marks(spans):
+    """rb_span_mark array of [(at, span_len), ...] (None when empty)."""
+    if not spans:
+        return None
+    return (capi.rb_span_mark * len(spans))(*[capi.rb_span_mark(int(at), int(span), 0) for at, span in spans])
 
 
 class _MixerShared:
