@@ -122,7 +122,8 @@ pub struct GpuSource {
 impl GpuSource {
     /// `SignalGenerator::new(sample_rate, frequency, f).take(n)` (src/source/signal_generator.rs:85-135); function: 0 sine,
     /// 1 triangle, 2 square, 3 sawtooth.  Nothing is uploaded: the samples are generated in HBM (f32 phase accumulation and
-    /// glibc's sinf bit for bit, like `f32::sin` on linux-gnu).
+    /// glibc's sinf bit for bit, like `f32::sin` on linux-gnu).  `n = u64::MAX` is the endless generator itself: a streaming
+    /// session generates it block by block until a `take_duration` in its chain or `rb_session_skip` ends it; it takes no pushes.
     pub fn signal_generator(sample_rate: SampleRate, frequency: f32, function: u32, n: u64) -> Self {
         assert!(frequency > 0.0, "frequency must be greater than zero");        // signal_generator.rs:112
         Self { pcm: vec![], channels: NonZero::new(1).unwrap(), sample_rate, span_len: 0, effects: vec![], reported_rate: sample_rate,

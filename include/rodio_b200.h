@@ -122,9 +122,11 @@ typedef enum {
                                  the SOURCE of the stream instead of uploaded PCM -- only as effects[0] of a descriptor with
                                  n_samples = 0, channels = 1, format f32, span_len = 0 (the generator reports None); generated on
                                  the device: f32 phase accumulation `phase = (phase + 1/(rate/freq)).rem_euclid(1.0)` and, for the
-                                 sine, glibc's sinf bit for bit (double-precision polynomial, restated in rb_kernels.cu).
+                                 sine, glibc's sinf bit for bit (double-precision polynomial, restated in rb_dsp.cuh).
                                  u32[0] = rb_signal_function, f32[0] = frequency (> 0 and finite: the reference asserts),
-                                 ns[0] = n, the number of samples taken from the endless generator             */
+                                 ns[0] = n, the number of samples taken from the endless generator.  In a streaming
+                                 session ns[0] = UINT64_MAX is the endless generator itself, and the session
+                                 generates the samples into the source's FIFO (see rb_session_create) */
 } rb_effect_kind;
 typedef enum { RB_SIGNAL_SINE = 0, RB_SIGNAL_TRIANGLE = 1, RB_SIGNAL_SQUARE = 2, RB_SIGNAL_SAWTOOTH = 3 } rb_signal_function;
                               /* src/source/signal_generator.rs:40-69 */
@@ -350,6 +352,16 @@ rb_status rb_batch_read_stream(rb_batch* b, size_t stream, float* out_host, uint
  * inside a frame; rb_session_create_ex with RB_SESSION_RESTARTS follows those restarts.  Sources of different shapes may share a
  * session (classes of their own); desc.n_samples / span_len are ignored (span_len: unless RB_SESSION_RESTARTS is given),
  * desc.mix_start is the mixer FRAME the source joins at.  Everything below counts frames; PCM is interleaved.
+ * GENERATOR SOURCES: a descriptor may begin with RB_FX_SIGNAL under the batch rules (effects[0], n_samples = 0, mono, f32,
+ * span_len = 0; the statuses of rb_stream_plan), followed by any chain above (push program, [SPEED | AMPLIFY | one filter]
+ * UNIFORM ...).  ns[0] = n: the source ends after n samples; UINT64_MAX: rodio's endless generator, ended by a TAKE_DURATION in
+ * its program or by rb_session_skip.  The session generates its samples on the device: a playing or held generator that has not
+ * ended holds min(fifo_frames, frames its take still lets through) input frames ahead of its converter, as if they had been pushed
+ * -- rb_session_available counts it so and rb_session_render generates what is missing before it plans the block -- so it never
+ * holds the mixer up.  It takes no pushes: rb_session_push(_spans) with frames, end_of_stream or marks and rb_session_push_packed
+ * (_spans) with a count, end_of_stream or mark for it return RB_ERR_STATE, rb_session_push_silence RB_ERR_UNSUPPORTED (a refused
+ * call changes nothing).  Every other call treats it as a pushed source with the same PCM: a session with generators renders the
+ * bytes of the same session whose generators are replaced by sources pushed with the generators' samples, for any split.
  * One caller per session; every call returns with the work done (the caller may reuse its buffers). */
 typedef struct rb_session rb_session;
 /* desc.mix_start of a source that is declared now but handed to the mixer later -- Mixer::add while the mixer is playing
@@ -458,7 +470,9 @@ rb_status rb_session_render(rb_session* s, float* out_host, uint64_t max_frames,
  * source is one row carrying all of its channels (mono and stereo mixers, mono sources in any mixer) writes version 5, any
  * other layout version 6 with a layout record per row; a session with push programs writes version 7, which adds the program
  * frames each source has consumed and the programs; a session with restart schedules writes version 8, which adds the converter
- * run of each source.  A blob of another shape, schedule, layout, master chain or program: RB_ERR_INVALID_ARGUMENT. */
+ * run of each source; a session with generator sources writes version 10: the blob it would otherwise write, then one record per
+ * generator (its phase, the samples it generated).  A blob of another shape, schedule, layout, master chain, program or generator
+ * set: RB_ERR_INVALID_ARGUMENT. */
 rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap, uint64_t* size);
 rb_status rb_session_set_state(rb_session* s, const void* buf, uint64_t size);
 

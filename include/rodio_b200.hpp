@@ -142,8 +142,9 @@ class Source {
         }
         return s;
     }
-    // SignalGenerator::new(sample_rate, frequency, function).take(n) -- signal_generator.rs:85-135: generated on the device
-    static Source signal_generator(uint32_t sample_rate, float frequency, rb_signal_function f, uint64_t n) {
+    // SignalGenerator::new(sample_rate, frequency, function).take(n) -- signal_generator.rs:85-135: generated on the device.
+    // n = UINT64_MAX (the default): the endless generator, which a LiveMixer plays until a take_duration or skip ends it.
+    static Source signal_generator(uint32_t sample_rate, float frequency, rb_signal_function f, uint64_t n = UINT64_MAX) {
         if (!(frequency > 0.0f)) throw std::invalid_argument("frequency must be greater than zero");   // :112
         Source s(1, sample_rate, {}, 0);
         s.effects_.push_back(fx(RB_FX_SIGNAL, {(uint32_t)f}, {frequency}, {n}));

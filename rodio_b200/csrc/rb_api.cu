@@ -1829,6 +1829,18 @@ struct rb_session {
     std::vector<uint64_t> report, none_cap;
     std::vector<uint8_t> follows_marks;        // the source is resampled in a session with RB_SESSION_RESTARTS: marks move its runs
     bool marked = false;
+    // generator sources (RB_FX_SIGNAL): the session generates their samples into their FIFOs before each render, as if they had been
+    // pushed.  Per source (source order) its phase slot (~0u: not a generator); per slot the source, the function, the phase step
+    // and the samples `.take(n)` lets through (~0: endless).  The phase of every generator's next sample lives on the device,
+    // double-buffered like the limiter state: a fill reads d_phase[phase_k] and writes d_phase[phase_k ^ 1], and phase_k flips once
+    // the render's synchronisation succeeded.  gen_frames: the samples the fill of the current render writes.
+    std::vector<uint32_t> gen_of, gens, gen_fn;
+    std::vector<float> gen_step;
+    std::vector<uint64_t> gen_end;
+    float* d_phase[2] = {nullptr, nullptr};
+    int phase_k = 0;
+    uint64_t gen_frames = 0;
+    rb_fifo_gen_job *d_gjobs = nullptr, *h_gjobs = nullptr;
 #if defined(RB_SIMT_EMULATE)
     std::vector<uint64_t> emu_fast_tiles;      // CPU build: fast tiles the emulator ran per class (rb_session_emu_fast_tiles)
 #endif
@@ -1843,6 +1855,7 @@ extern "C" rb_status rb_session_destroy(rb_session* s) {
     cudaFree(s->d_master[0]), cudaFree(s->d_master[1]), cudaFree(s->d_master_runs), cudaFreeHost(s->h_master_runs);
     cudaFree(s->d_prog), cudaFree(s->d_pjobs), cudaFreeHost(s->h_pjobs);
     cudaFree(s->d_cuts), cudaFreeHost(s->h_cuts), cudaFree(s->d_cut_first), cudaFreeHost(s->h_cut_first);
+    cudaFree(s->d_phase[0]), cudaFree(s->d_phase[1]), cudaFree(s->d_gjobs), cudaFreeHost(s->h_gjobs);
     delete s;
     return RB_OK;
 }
@@ -1876,26 +1889,44 @@ extern "C" rb_status rb_session_create_ex(rb_context* ctx, uint16_t mixer_channe
     std::vector<uint8_t> no_silence(n, 0);
     std::vector<uint64_t> run_cap(n, 0);      // RB_SESSION_RESTARTS: frames per converter run (0: the source is one run)
     std::vector<uint64_t> none_cap(n, session::NO_LIMIT);   // ... under a report of None
+    std::vector<float> gen_step(n, 0.0f);     // generator sources: their phase step (gen[i])
+    std::vector<uint8_t> gen(n, 0);
     for (size_t i = 0; i < n; i++) {
         const rb_stream_desc& d = descs[i];
         const std::string where = "stream " + std::to_string(i) + ": ";
         if (d.sample_rate == 0 || d.channels == 0) return fail(RB_ERR_INVALID_ARGUMENT, where + "zero sample rate or channels");
+        if (d.n_effects && !d.effects) return fail(RB_ERR_INVALID_ARGUMENT, where + "effects is NULL");
+        for (uint32_t k = 1; k < d.n_effects; k++)
+            if (d.effects[k].kind == RB_FX_SIGNAL)
+                return fail(RB_ERR_INVALID_ARGUMENT, where + "signal generator: only as effects[0] of an empty mono f32 span-less descriptor");
+        gen[i] = d.n_effects && d.effects[0].kind == RB_FX_SIGNAL;
+        if (gen[i]) {   // SignalGenerator::with_function (signal_generator.rs:107-128), validated as plan_stream does
+            const rb_effect& e = d.effects[0];
+            if (d.n_samples != 0 || d.channels != 1 || d.format != RB_FMT_F32 || d.span_len != 0)
+                return fail(RB_ERR_INVALID_ARGUMENT, where + "signal generator: only as effects[0] of an empty mono f32 span-less descriptor");
+            if (e.u32[0] > RB_SIGNAL_SAWTOOTH) return fail(RB_ERR_INVALID_ARGUMENT, where + "signal generator: unknown function");
+            if (!(e.f32[0] > 0.0f)) return fail(RB_ERR_INVALID_ARGUMENT, where + "signal generator: frequency must be greater than zero");
+            if (!std::isfinite(e.f32[0])) return fail(RB_ERR_UNSUPPORTED, where + "signal generator: infinite frequency");
+            volatile float period = (float)d.sample_rate / e.f32[0];     // :118, the expression plan_stream uses
+            gen_step[i] = 1.0f / period;                                 // :119
+        }
         if (d.format != RB_FMT_F32) return fail(RB_ERR_UNSUPPORTED, where + "sessions take f32 sources");
         if (d.channels > RB_MAX_CHANNELS) return fail(RB_ERR_UNSUPPORTED, where + "more than 12 channels");
         if (mixer_channels == 1 && d.channels != 1) return fail(RB_ERR_UNSUPPORTED, where + "a mono mixer takes mono sources");
         chs[i] = d.channels;
-        if (d.n_effects && !d.effects) return fail(RB_ERR_INVALID_ARGUMENT, where + "effects is NULL");
         // The push program: effects [0, p), p one past the last LINEAR_RAMP / TAKE_DURATION / DISTORTION in front of everything
         // else.  No state depends on the signal there: every output sample is a function of its input sample and its index in
         // the source, so the scatter of each push applies them.  Each one sees the rate the SPEEDs in front of it report.
-        uint32_t p = 0, rate = d.sample_rate;
-        for (uint32_t k = 0; k < d.n_effects; k++) {
+        // A generator is the source itself: what follows it is a chain as for pushed PCM.
+        const uint32_t k_src = gen[i] ? 1u : 0u;
+        uint32_t p = k_src, rate = d.sample_rate;
+        for (uint32_t k = k_src; k < d.n_effects; k++) {
             const uint32_t kd = d.effects[k].kind;
             if (kd == RB_FX_LINEAR_RAMP || kd == RB_FX_TAKE_DURATION || kd == RB_FX_DISTORTION) p = k + 1;
             else if (kd != RB_FX_AMPLIFY && kd != RB_FX_SPEED) break;
         }
         bool take_open = false;   // ops behind a take that ends inside a frame see its 0.0 padding
-        for (uint32_t k = 0; k < p; k++) {
+        for (uint32_t k = k_src; k < p; k++) {
             const rb_effect& e = d.effects[k];
             if (e.kind == RB_FX_SPEED) {
                 rate = rb_speed_sample_rate(rate, e.f32[0]);
@@ -1996,6 +2027,7 @@ extern "C" rb_status rb_session_create_ex(rb_context* ctx, uint16_t mixer_channe
     s->vol_a.assign(n, 1.0f), s->vol_b.assign(n, 1.0f), s->pads.assign(n, 0);
     s->prog_op0.assign(n, 0), s->prog_n.assign(n, 0), s->prog_pos.assign(n, 0), s->prog_end.assign(n, ~0ull), s->no_silence.assign(n, 0);
     s->restarts = restarts, s->report.assign(n, 0), s->none_cap.assign(n, session::NO_LIMIT), s->follows_marks.assign(n, 0);
+    s->gen_of.assign(n, ~0u);
     bool any_biquad = false;
     std::vector<uint8_t> row_ff2(n, 1);
     for (size_t r = 0; r < n; r++) {
@@ -2053,6 +2085,12 @@ extern "C" rb_status rb_session_create_ex(rb_context* ctx, uint16_t mixer_channe
         if (take_n[i] != ~0ull) {   // the take's last frame, padded: the source ends there
             s->prog_end[r] = (take_n[i] + d.channels - 1) / d.channels;
             if (s->prog_end[r] == 0) s->st[r].eof = true;
+        }
+        s->gen_of[r] = gen[i] ? (uint32_t)s->gens.size() : ~0u;
+        if (gen[i]) {   // ns[0]: `.take(n)`, the samples the source has; UINT64_MAX: the endless generator
+            s->gens.push_back((uint32_t)r), s->gen_fn.push_back(d.effects[0].u32[0]), s->gen_step.push_back(gen_step[i]);
+            s->gen_end.push_back(d.effects[0].ns[0]);
+            if (d.effects[0].ns[0] == 0) s->st[r].eof = true;
         }
     }
     s->has_prog = !s->prog_ops.empty();
@@ -2133,6 +2171,13 @@ extern "C" rb_status rb_session_create_ex(rb_context* ctx, uint16_t mixer_channe
         RB_CUDA(cudaMallocHost(&s->h_pjobs, nr * sizeof(rb_fifo_prog_job)));
         RB_CUDA(cudaMemcpyAsync(s->d_prog, s->prog_ops.data(), s->prog_ops.size() * sizeof(rb_prog_op), cudaMemcpyHostToDevice, ctx->stream));
     }
+    if (!s->gens.empty()) {   // every generator starts at phase 0.0 (signal_generator.rs:126)
+        const size_t ng = s->gens.size();
+        for (int k = 0; k < 2; k++) RB_CUDA(cudaMalloc(&s->d_phase[k], ng * sizeof(float)));
+        RB_CUDA(cudaMalloc(&s->d_gjobs, ng * sizeof(rb_fifo_gen_job)));
+        RB_CUDA(cudaMallocHost(&s->h_gjobs, ng * sizeof(rb_fifo_gen_job)));
+        RB_CUDA(cudaMemsetAsync(s->d_phase[0], 0, ng * sizeof(float), ctx->stream));
+    }
     RB_CUDA(cudaStreamSynchronize(ctx->stream));
     *out = s.release();
     return RB_OK;
@@ -2182,6 +2227,35 @@ static void session_pushed(rb_session* s, size_t r, uint64_t frames, const std::
     s->prog_pos[r] += frames;
     if (session_take_ended(s, r)) s->st[r].eof = true;
 }
+// Generators that have not ended hold what their FIFO takes, as far as their take and `.take(n)` let them through, as if those
+// frames had been pushed: every generator's share of the next fill goes into h_gjobs (frames 0: its phase passes through) and
+// through session_pushed; gen_frames counts the samples.  Host bookkeeping only -- session_render_block launches the fill, and
+// callers that do not render put the streams back (session_gen_undo).
+struct SessionGenUndo {
+    std::vector<session::Stream> st;
+    std::vector<uint64_t> prog_pos;
+    bool has_sched = false;
+};
+static SessionGenUndo session_gen_top_up(rb_session* s) {
+    SessionGenUndo u;
+    s->gen_frames = 0;
+    if (s->gens.empty()) return u;
+    u.st = s->st, u.prog_pos = s->prog_pos, u.has_sched = s->has_sched;
+    for (uint32_t g = 0; g < (uint32_t)s->gens.size(); g++) {
+        const size_t r = s->gens[g];
+        session::Stream& st = s->st[r];
+        const uint64_t k = st.eof ? 0 : std::min({(uint64_t)s->fifo_cap - st.fill(), session_take_left(s, r), s->gen_end[g] - s->prog_pos[r]});
+        s->h_gjobs[g] = rb_fifo_gen_job{s->prog_pos[r], s->rows_of[r][0], (uint32_t)st.fill(), (uint32_t)k, g, s->prog_op0[r], s->prog_n[r], s->gen_fn[g], s->gen_step[g]};
+        if (k) session_pushed(s, r, k);
+        if (s->prog_pos[r] >= s->gen_end[g]) st.eof = true;
+        s->gen_frames += k;
+    }
+    return u;
+}
+static void session_gen_undo(rb_session* s, SessionGenUndo& u) {
+    if (s->gens.empty()) return;
+    s->st = std::move(u.st), s->prog_pos = std::move(u.prog_pos), s->has_sched = u.has_sched, s->gen_frames = 0;
+}
 // The run cap (frames) a report of `span_len` samples gives source r (source order): min(span_len, 32768) samples
 // (src/source/uniform.rs:55), BAD_CAP when that is not whole frames or under two; for None the take's cap, or none.
 static uint64_t session_report_cap(const rb_session* s, size_t r, uint64_t span_len) {
@@ -2219,6 +2293,7 @@ static rb_status session_push_one(rb_session* s, size_t stream, const float* pcm
     if (!s || (!pcm && n_frames)) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
     if (stream >= s->st.size()) return fail(RB_ERR_INVALID_ARGUMENT, "stream index out of range");
     stream = s->pos[stream];   // class order from here on
+    if (s->gen_of[stream] != ~0u && (n_frames || n_marks || end_of_stream)) return fail(RB_ERR_STATE, "a generator source takes no pushes");
     session::Stream& st = s->st[stream];
     std::vector<session::CapChange> changes;
     rb_status rc = session_span_changes(s, stream, n_frames, marks, n_marks, &changes);
@@ -2257,6 +2332,8 @@ extern "C" rb_status rb_session_push_silence(rb_session* s, size_t stream, uint6
     if (stream >= s->st.size()) return fail(RB_ERR_INVALID_ARGUMENT, "stream index out of range");
     const size_t r = s->pos[stream];
     session::Stream& st = s->st[r];
+    if (s->gen_of[r] != ~0u)   // its FIFO runs ahead of the converter: zeros appended there would land fifo_frames late
+        return fail(RB_ERR_UNSUPPORTED, "silence into a generator source");
     if (st.front)   // rodio does not pull that filter while paused; the render would run it over the zeros
         return fail(RB_ERR_UNSUPPORTED, "silence into a source with a filter in front of the conversion");
     if (s->no_silence[r] && !st.eof)   // rodio's conversion counts the zeros against the take's span and restarts early
@@ -2287,6 +2364,8 @@ static rb_status session_push_many(rb_session* s, const float* pcm, const uint64
     std::vector<std::vector<session::CapChange>> changes(n_marks ? ns : 0);
     for (size_t i = 0, m = 0; i < ns; i++) {   // i: the caller's index, pos[i]: class order
         const session::Stream& st = s->st[s->pos[i]];
+        if (s->gen_of[s->pos[i]] != ~0u && (n_frames[i] || (end_of_stream && end_of_stream[i]) || (n_marks && n_marks[i])))
+            return fail(RB_ERR_STATE, "stream " + std::to_string(i) + ": a generator source takes no pushes");
         if (n_marks) {
             rb_status rc = session_span_changes(s, s->pos[i], n_frames[i], marks ? marks + m : nullptr, n_marks[i], &changes[i]);
             if (rc != RB_OK) return fail(rc, "stream " + std::to_string(i) + ": " + rb_last_error());
@@ -2423,9 +2502,11 @@ extern "C" rb_status rb_session_set_master(rb_session* s, const rb_effect* effec
 extern "C" rb_status rb_session_available(rb_session* s, uint64_t* frames, int* ended) {
     if (!s || !frames) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
     bool e = false;
+    SessionGenUndo u = session_gen_top_up(s);   // generators count with the frames the next render gives them
     session::resolve_queue(s->st, s->T);
     *frames = session::renderable(s->st, s->T, ~0ull >> 1, &e);
     if (ended) *ended = e ? 1 : 0;
+    session_gen_undo(s, u);
     return RB_OK;
 }
 
@@ -2435,15 +2516,22 @@ extern "C" rb_status rb_session_render(rb_session* s, float* out_host, uint64_t 
     if (!s || !written) return fail(RB_ERR_INVALID_ARGUMENT, "NULL argument");
     *written = 0;
     bool e = false;
+    SessionGenUndo u = session_gen_top_up(s);   // generators first: a generator never holds the mixer up
     session::resolve_queue(s->st, s->T);   // queued sources whose predecessor's end is known by now get their place on the timeline
     const uint64_t n = session::renderable(s->st, s->T, std::min<uint64_t>(max_frames, s->max_block), &e);
     if (ended) *ended = e ? 1 : 0;
-    if (n == 0) return RB_OK;
-    if (!out_host) return fail(RB_ERR_INVALID_ARGUMENT, "out_host is NULL");
+    if (n == 0 || !out_host) {   // nothing is rendered: the generators are topped up by the render that is
+        session_gen_undo(s, u);
+        return n == 0 ? RB_OK : fail(RB_ERR_INVALID_ARGUMENT, "out_host is NULL");
+    }
     if (s->has_sched)
         for (session::Stream& st : s->st) session::settle(st);
     rb_status rc = session_render_block(s, out_host, n);
-    if (rc != RB_OK) return rc;
+    if (rc != RB_OK) {
+        session_gen_undo(s, u);
+        return rc;
+    }
+    if (s->gen_frames) s->phase_k ^= 1, s->gen_frames = 0;
     *written = n;
     if (ended) {
         bool e2 = false;
@@ -2512,6 +2600,11 @@ static rb_status session_render_block(rb_session* s, float* out_host, uint64_t n
         row.f0 = s->st[r].fpos - s->st[r].i0, row.ga = s->vol_a[r], row.gb = s->vol_b[r];
     }
     RB_CUDA(cudaMemcpyAsync(s->d_rows, s->h_rows, nr * sizeof(lanes::Row), cudaMemcpyHostToDevice, stq));
+    if (s->gen_frames) {   // the generators' new frames (session_gen_top_up), in front of the kernels that read them
+        const uint32_t ng = (uint32_t)s->gens.size();
+        RB_CUDA(cudaMemcpyAsync(s->d_gjobs, s->h_gjobs, ng * sizeof(rb_fifo_gen_job), cudaMemcpyHostToDevice, stq));
+        RB_CUDA(rb_lanes_fifo_generate(s->d_gjobs, ng, s->d_prog, s->d_phase[s->phase_k], s->d_phase[s->phase_k ^ 1], fifo, s->stride, s->d_flags, stq));
+    }
     if (any_cut) {
         RB_CUDA(cudaMemcpyAsync(s->d_cuts, s->h_cuts, n_cuts * sizeof(lanes::Cut), cudaMemcpyHostToDevice, stq));
         RB_CUDA(cudaMemcpyAsync(s->d_cut_first, s->h_cut_first, (nr + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stq));
@@ -2679,6 +2772,17 @@ struct SessionBlobProg {
 struct SessionBlobRun {
     uint64_t run_cap, run_i, run_o, sched_end, runs_done, n_ends;
 };
+// Version 10 (a session with generator sources): the blob the session would otherwise write (version 5 to 9, with 10 in its
+// header), then one record per generator (phase slot order) and a tail with the version that record carries.  A blob only restores
+// a session with the same generators; sessions without generators never write or take version 10.
+struct SessionBlobGen {
+    uint32_t src, fn;                    // source order; rb_signal_function
+    float step, phase;                   // the phase step; the phase of its next sample
+    uint64_t generated, end;             // samples generated so far; ns[0] of its descriptor
+};
+struct SessionBlobGenTail {              // the blob's last bytes
+    uint32_t version, n_gens;
+};
 constexpr uint32_t SESSION_MAGIC = 0x52425353u;   // "RBSS"
 uint32_t blob_version(const rb_session* s) { return s->marked ? 9u : s->has_sched ? 8u : s->has_prog ? 7u : s->plain ? 5u : 6u; }
 uint64_t blob_run_bytes(const rb_session* s) {
@@ -2705,6 +2809,8 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
     const uint32_t C = s->channels;
     for (size_t q = 0; q < nr; q++) need += s->st[s->rows[q].src].fill() * s->rows[q].ci * sizeof(float);
     if (s->has_master) need += sizeof(SessionBlobMaster);
+    const uint64_t inner = need, ng = s->gens.size();
+    if (ng) need += ng * sizeof(SessionBlobGen) + sizeof(SessionBlobGenTail);
     *size = need;
     if (!buf) return RB_OK;
     if (cap < need) return fail(RB_ERR_BUFFER_TOO_SMALL, "state buffer too small");
@@ -2716,8 +2822,10 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
     float mstate[2 * RB_MAX_CHANNELS] = {0};
     if (s->has_master)
         RB_CUDA(cudaMemcpyAsync(mstate, s->d_master[s->master_k], 2 * C * sizeof(float), cudaMemcpyDeviceToHost, s->ctx->stream));
+    std::vector<float> phase(ng);
+    if (ng) RB_CUDA(cudaMemcpyAsync(phase.data(), s->d_phase[s->phase_k], ng * sizeof(float), cudaMemcpyDeviceToHost, s->ctx->stream));
     uint8_t* p = (uint8_t*)buf;
-    SessionBlobHeader h{SESSION_MAGIC, blob_version(s), (uint32_t)nr, s->has_biquad ? 1u : 0u, C, s->has_master ? 1u : 0u, s->T};
+    SessionBlobHeader h{SESSION_MAGIC, ng ? 10u : blob_version(s), (uint32_t)nr, s->has_biquad ? 1u : 0u, C, s->has_master ? 1u : 0u, s->T};
     memcpy(p, &h, sizeof(h)), p += sizeof(h);
     uint8_t* recs = p;
     p += nr * sizeof(SessionBlobStream);
@@ -2761,6 +2869,16 @@ extern "C" rb_status rb_session_get_state(rb_session* s, void* buf, uint64_t cap
         for (uint32_t c = 0; c < C; c++) m.integ[c] = mstate[c], m.peak[c] = mstate[C + c];
         memcpy(p, &m, sizeof(m));
     }
+    if (ng) {
+        p = (uint8_t*)buf + inner;
+        for (uint32_t g = 0; g < ng; g++) {
+            const uint32_t r = s->gens[g];
+            const SessionBlobGen b{r, s->gen_fn[g], s->gen_step[g], phase[g], s->prog_pos[r], s->gen_end[g]};
+            memcpy(p, &b, sizeof(b)), p += sizeof(b);
+        }
+        const SessionBlobGenTail tail{blob_version(s), (uint32_t)ng};
+        memcpy(p, &tail, sizeof(tail));
+    }
     return RB_OK;
 }
 
@@ -2773,6 +2891,29 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
     if (size < sizeof(h)) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
     memcpy(&h, p, sizeof(h)), p += sizeof(h);
     const uint32_t C = s->channels;
+    // version 10: the generator records and the tail come off the end, the rest is read as the version the tail names
+    const size_t ng = s->gens.size();
+    const bool v10 = h.magic == SESSION_MAGIC && h.version == 10u;
+    if (v10 != (ng != 0) && h.magic == SESSION_MAGIC && h.version >= 5u && h.version <= 10u)
+        return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session with other generator sources");
+    std::vector<SessionBlobGen> gens(ng);
+    if (v10) {
+        const uint64_t tail_bytes = ng * sizeof(SessionBlobGen) + sizeof(SessionBlobGenTail);
+        if (size < sizeof(h) + tail_bytes) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
+        SessionBlobGenTail tail;
+        memcpy(&tail, (const uint8_t*)buf + size - sizeof(tail), sizeof(tail));
+        if (tail.n_gens != ng) return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session with other generator sources");
+        size -= tail_bytes;
+        memcpy(gens.data(), (const uint8_t*)buf + size, ng * sizeof(SessionBlobGen));
+        for (size_t g = 0; g < ng; g++) {
+            const SessionBlobGen& b = gens[g];
+            if (b.src != s->gens[g] || b.fn != s->gen_fn[g] || memcmp(&b.step, &s->gen_step[g], sizeof(float)) || b.end != s->gen_end[g] ||
+                b.generated > b.end || !(b.phase >= 0.0f && b.phase < 1.0f))
+                return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session with other generator sources");
+        }
+        h.version = tail.version;
+        if (h.version == 10u) return fail(RB_ERR_INVALID_ARGUMENT, "not a session state blob");
+    }
     if (h.magic != SESSION_MAGIC || h.version < 5u || h.version > 9u) return fail(RB_ERR_INVALID_ARGUMENT, "not a session state blob");
     // a version-9 blob (span marks) restores into a session of the same shape with RB_SESSION_RESTARTS, marked or not
     const bool v9 = h.version == 9u;
@@ -2860,6 +3001,10 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
             return fail(RB_ERR_INVALID_ARGUMENT, "state blob belongs to a session with another master chain");
     }
     if (size < need) return fail(RB_ERR_INVALID_ARGUMENT, "state blob truncated");
+    if (v10 && size != need) return fail(RB_ERR_INVALID_ARGUMENT, "state blob: generator records out of place");
+    for (size_t g = 0; g < ng; g++)   // a generator has received what it generated, less what a skip dropped
+        if (recs[s->rows_of[s->gens[g]][0]].pushed > gens[g].generated)
+            return fail(RB_ERR_INVALID_ARGUMENT, "state blob: a generator holds more frames than it generated");
     RB_CUDA(cudaSetDevice(s->ctx->device));
     std::vector<float> state(8 * nr);
     std::vector<uint32_t> flags(nr);
@@ -2891,9 +3036,13 @@ extern "C" rb_status rb_session_set_state(rb_session* s, const void* buf, uint64
         for (uint32_t c = 0; c < C; c++) mstate[c] = m.integ[c], mstate[C + c] = m.peak[c];
         RB_CUDA(cudaMemcpyAsync(s->d_master[s->master_k], mstate, 2 * C * sizeof(float), cudaMemcpyHostToDevice, s->ctx->stream));
     }
+    std::vector<float> phase(ng);
+    for (size_t g = 0; g < ng; g++) phase[g] = gens[g].phase;
+    if (ng) RB_CUDA(cudaMemcpyAsync(s->d_phase[s->phase_k], phase.data(), ng * sizeof(float), cudaMemcpyHostToDevice, s->ctx->stream));
     RB_CUDA(cudaStreamSynchronize(s->ctx->stream));
     s->T = h.T;
     if (s->has_prog) s->prog_pos = prog_pos;
+    for (size_t g = 0; g < ng; g++) s->prog_pos[s->gens[g]] = gens[g].generated;
     if (v9) s->report = report, s->marked = true;
     return RB_OK;
 }

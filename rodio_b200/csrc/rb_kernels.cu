@@ -78,55 +78,6 @@ __global__ void __launch_bounds__(TPB) k_delay(const rb_node_dev* __restrict__ n
 }
 
 // ---------------------------------------------------------------- signal generators (a source, src/source/signal_generator.rs)
-// glibc's sinf for arguments in [0, 2*pi] -- what `(TAU * phase).sin()` (signal_generator.rs:51-53) resolves to on linux-gnu:
-// the argument widened to double, one multiply-subtract of range reduction into [-pi/4, pi/4] with the quadrant, a degree-7
-// (sine) or degree-8 (cosine) polynomial in double, one rounding to float.  The coefficients are the published ones of glibc
-// >= 2.28 (sysdeps/ieee754/flt-32/sincosf_data.c); the restatement was held against the libm of this image on every float of
-// [0, 0x40c90fdb] (tools/microbench/sinf_exhaustive.cpp: 1 086 918 620 arguments, 0 mismatches, with and without contraction of
-// the double multiply-adds -- so the ifunc variant libm picks on the host does not matter).  FP64 here is IEEE: bit for bit.
-__device__ __forceinline__ float sinf_glibc_0_tau(float y) {
-    const double x = (double)y;
-    const uint32_t top = (__float_as_uint(y) >> 20) & 0x7ffu;
-    double xr, x2, sgn = 1.0;
-    int n = 0;
-    if (top < 0x3f4u) {                      // |y| < pi/4 (abstop12 of 0x1.921FB6p-1f)
-        if (top < 0x398u) return y;          // |y| < 2^-12
-        xr = x, x2 = __dmul_rn(x, x);
-    } else {
-        const double r = __dmul_rn(x, 0x1.45F306DC9C883p+23);               // 2/pi * 2^24
-        n = (__double2int_rz(r) + 0x800000) >> 24;
-        xr = __dsub_rn(x, __dmul_rn((double)n, 0x1.921FB54442D18p0));       // pi/2
-        sgn = (n & 3) == 1 || (n & 3) == 2 ? -1.0 : 1.0;                     // sign[n & 3] = {1, -1, -1, 1}
-        x2 = __dmul_rn(xr, xr);
-        xr = __dmul_rn(xr, sgn);
-    }
-    const bool neg = (n & 2) != 0;           // second table: the cosine coefficients negated
-    if ((n & 1) == 0) {
-        const double s1c = -0x1.555545995a603p-3, s2c = 0x1.1107605230bc4p-7, s3c = -0x1.994eb3774cf24p-13;
-        const double x3 = __dmul_rn(xr, x2);
-        const double s1 = __dadd_rn(s2c, __dmul_rn(x2, s3c));
-        const double x7 = __dmul_rn(x3, x2);
-        const double s = __dadd_rn(xr, __dmul_rn(x3, s1c));
-        return __double2float_rn(__dadd_rn(s, __dmul_rn(x7, s1)));
-    }
-    const double k = neg ? -1.0 : 1.0;
-    const double c0 = k, c1 = k * -0x1.ffffffd0c621cp-2, c2k = k * 0x1.55553e1068f19p-5, c3 = k * -0x1.6c087e89a359dp-10,
-                 c4 = k * 0x1.99343027bf8c3p-16;
-    const double x4 = __dmul_rn(x2, x2);
-    const double c2 = __dadd_rn(c3, __dmul_rn(x2, c4));
-    const double c1v = __dadd_rn(c0, __dmul_rn(x2, c1));
-    const double x6 = __dmul_rn(x4, x2);
-    const double c = __dadd_rn(c1v, __dmul_rn(x4, c2k));
-    return __double2float_rn(__dadd_rn(c, __dmul_rn(x6, c2)));
-}
-__device__ __forceinline__ float signal_value(uint32_t fn, float phase) {   // signal_generator.rs:51-69
-    switch (fn) {
-        case RB_SIGNAL_SINE: return sinf_glibc_0_tau(mul(6.2831855f, phase));
-        case RB_SIGNAL_TRIANGLE: return sub(mul(4.0f, fabsf(sub(phase, floorf(add(phase, 0.5f))))), 1.0f);
-        case RB_SIGNAL_SQUARE: return phase < 0.5f ? 1.0f : -1.0f;           // phase % 1.0 == phase inside [0, 1)
-        default: return mul(2.0f, sub(phase, floorf(add(phase, 0.5f))));
-    }
-}
 // A CTA owns SIG_GENS generators (4: the waveform -- ~100 instructions per sine -- is what the seven worker warps have to keep up
 // with; with 32 generators per CTA the first version spent 220 cycles per sample step on 32 SMs, with 8 still 29).  The phase is a serial f32 recurrence per generator (`phase = (phase + step).rem_euclid(1.0)`,
 // signal_generator.rs:133: it drifts by design, so it cannot be computed from the sample index): warp 0, lane = generator, walks
@@ -151,14 +102,12 @@ __global__ void __launch_bounds__(SIG_THREADS) k_siggen(const rb_node_dev* __res
 #pragma unroll 8
                     for (int t = 0; t < SIG_TILE; t++) {
                         row[t] = phase;
-                        const float q = add(phase, step);            // < 2: q % 1.0 is q or q - 1, both exact
-                        phase = q >= 1.0f ? sub(q, 1.0f) : q;
+                        phase = signal_phase_next<true>(phase, step);
                     }
                 } else {
                     for (int t = 0; t < SIG_TILE; t++) {
                         row[t] = phase;
-                        const float q = add(phase, step);
-                        phase = sub(q, floorf(q));                    // q >= 0: fmodf(q, 1.0f) exactly
+                        phase = signal_phase_next<false>(phase, step);
                     }
                 }
             }

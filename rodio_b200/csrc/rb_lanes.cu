@@ -312,6 +312,64 @@ __global__ void __launch_bounds__(128) k_fifo_scatter(const float* __restrict__ 
     if (__syncthreads_or(bad ? 1 : 0) && threadIdx.x == 0) flags[j.row] = 1u;
 }
 
+// Generator fill (rb_lanes.h: rb_fifo_gen_job), k_siggen's shape (rb_kernels.cu): GEN_PER_CTA generators per CTA.  The phase is a
+// serial f32 recurrence that drifts by design (signal_generator.rs:133), so warp 0, lane = generator, walks exactly `frames` steps of
+// it a tile ahead into shared memory; the seven other warps evaluate the waveform of the previous tile, run the program, classify
+// and store with consecutive threads on consecutive samples.
+constexpr int GEN_TILE = 256, GEN_THREADS = 256, GEN_PITCH = GEN_TILE + 1, GEN_PER_CTA = 4;
+__global__ void __launch_bounds__(GEN_THREADS) k_fifo_generate(const rb_fifo_gen_job* __restrict__ jobs, uint32_t n_jobs,
+                                                               const rb_prog_op* __restrict__ ops, const float* __restrict__ phase_in,
+                                                               float* __restrict__ phase_out, float* __restrict__ fifo, uint64_t stride,
+                                                               uint32_t* __restrict__ flags) {
+    __shared__ float s_phase[2][GEN_PER_CTA * GEN_PITCH];
+    __shared__ rb_fifo_gen_job s_job[GEN_PER_CTA];
+    __shared__ uint32_t s_bad;
+    const uint32_t j0 = blockIdx.x * GEN_PER_CTA, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t n_g = min((uint32_t)GEN_PER_CTA, n_jobs - j0);
+    if (threadIdx.x < n_g) s_job[threadIdx.x] = jobs[j0 + threadIdx.x];
+    if (threadIdx.x == 0) s_bad = 0;
+    __syncthreads();
+    uint32_t max_n = 0;
+    for (uint32_t g = 0; g < n_g; g++) max_n = max(max_n, s_job[g].frames);
+    const uint32_t n_tiles = (max_n + GEN_TILE - 1) / GEN_TILE;
+    float phase = 0.0f;
+    if (warp == 0 && lane < n_g) phase = phase_in[s_job[lane].gen];
+    uint32_t bad = 0;   // worker threads: bit g = a sample of generator g lies outside the exact-reciprocal class
+    for (uint32_t it = 0; it <= n_tiles; it++) {
+        if (warp == 0) {
+            const uint32_t lo = it * GEN_TILE;
+            if (it < n_tiles && lane < n_g && lo < s_job[lane].frames) {
+                float* row = &s_phase[it & 1][lane * GEN_PITCH];
+                const uint32_t cnt = min((uint32_t)GEN_TILE, s_job[lane].frames - lo);
+                const float step = s_job[lane].step;
+                if (step < 1.0f) {
+#pragma unroll 8
+                    for (uint32_t t = 0; t < cnt; t++) row[t] = phase, phase = rbd::signal_phase_next<true>(phase, step);
+                } else {
+                    for (uint32_t t = 0; t < cnt; t++) row[t] = phase, phase = rbd::signal_phase_next<false>(phase, step);
+                }
+            }
+        } else if (it > 0) {
+            const uint32_t lo = (it - 1) * GEN_TILE;
+            for (uint32_t w = threadIdx.x - 32; w < n_g * GEN_TILE; w += GEN_THREADS - 32) {
+                const uint32_t g = w / GEN_TILE, t = w % GEN_TILE;
+                const rb_fifo_gen_job& j = s_job[g];
+                if (lo + t >= j.frames) continue;
+                float v = rbd::signal_value(j.fn, s_phase[(it - 1) & 1][g * GEN_PITCH + t]);
+                v = run_prog(v, j.base + lo + t, 1, ops + j.op0, j.n_ops);
+                const uint32_t u = __float_as_uint(v) & 0x7fffffffu;
+                if (u != 0u && (u - 0x1c800000u) >= (0x5d800000u - 0x1c800000u)) bad |= 1u << g;
+                fifo[(uint64_t)j.row * stride + j.fill + lo + t] = v;
+            }
+        }
+        __syncthreads();
+    }
+    if (bad) atomicOr(&s_bad, bad);
+    if (warp == 0 && lane < n_g) phase_out[s_job[lane].gen] = phase;
+    __syncthreads();
+    if (threadIdx.x < n_g && ((s_bad >> threadIdx.x) & 1u)) flags[s_job[threadIdx.x].row] = 1u;
+}
+
 __global__ void __launch_bounds__(128) k_fifo_compact(const float* __restrict__ src, float* __restrict__ dst, uint64_t stride,
                                                       const uint32_t* __restrict__ drop, const uint32_t* __restrict__ keep) {
     const uint32_t r = blockIdx.x, n = keep[r];
@@ -469,6 +527,13 @@ cudaError_t rb_lanes_fifo_scatter_prog(const float* d_staging, const rb_fifo_pro
                                        float* d_fifo, uint64_t stride, uint32_t* d_flags, cudaStream_t st) {
     if (n_jobs == 0) return cudaSuccess;
     k_fifo_scatter<true><<<n_jobs, 128, 0, st>>>(d_staging, d_jobs, d_fifo, stride, d_flags, d_ops);
+    return cudaGetLastError();
+}
+
+cudaError_t rb_lanes_fifo_generate(const rb_fifo_gen_job* d_jobs, uint32_t n_jobs, const rb_prog_op* d_ops, const float* d_phase_in,
+                                   float* d_phase_out, float* d_fifo, uint64_t stride, uint32_t* d_flags, cudaStream_t st) {
+    if (n_jobs == 0) return cudaSuccess;
+    k_fifo_generate<<<(n_jobs + GEN_PER_CTA - 1) / GEN_PER_CTA, GEN_THREADS, 0, st>>>(d_jobs, n_jobs, d_ops, d_phase_in, d_phase_out, d_fifo, stride, d_flags);
     return cudaGetLastError();
 }
 

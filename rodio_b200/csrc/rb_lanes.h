@@ -120,6 +120,21 @@ struct rb_fifo_prog_job {     // a job of a session with push programs, 40 bytes
 // chain order, and classified after it.
 cudaError_t rb_lanes_fifo_scatter_prog(const float* d_staging, const rb_fifo_prog_job* d_jobs, uint32_t n_jobs, const rb_prog_op* d_ops,
                                        float* d_fifo, uint64_t stride, uint32_t* d_flags, cudaStream_t st);
+// ---- generator sources (RB_FX_SIGNAL): the session writes their samples into the FIFO itself, before each render ----
+struct rb_fifo_gen_job {      // one generator, 40 bytes
+    uint64_t base;            // samples it has generated so far: the index of its next sample in the source and its program
+    uint32_t row, fill;       // its row (mono: one per generator) and the frames already in that row's FIFO
+    uint32_t frames;          // samples to generate now (0: the phase passes through unchanged)
+    uint32_t gen;             // its phase slot
+    uint32_t op0, n_ops;      // its push program: ops[op0, op0 + n_ops)
+    uint32_t fn;              // rb_signal_function
+    float step;               // 1 / (rate / frequency) in f32 (signal_generator.rs:118-119)
+};
+// Generator fill: job k writes samples [base, base + frames) of its generator behind the row's fill frames -- the phase recurrence
+// from phase_in[gen], the waveform, the program, the sticky classification into flags[row] -- and leaves the phase of its next
+// sample in phase_out[gen].  A few generators per CTA; every job, with or without frames, writes its phase_out.
+cudaError_t rb_lanes_fifo_generate(const rb_fifo_gen_job* d_jobs, uint32_t n_jobs, const rb_prog_op* d_ops, const float* d_phase_in,
+                                   float* d_phase_out, float* d_fifo, uint64_t stride, uint32_t* d_flags, cudaStream_t st);
 // FIFO compaction into the other arena: dst[r][0, keep[r]) = src[r][drop[r], drop[r] + keep[r]).
 cudaError_t rb_lanes_fifo_compact(const float* d_src, float* d_dst, uint64_t stride, const uint32_t* d_drop, const uint32_t* d_keep,
                                   uint32_t n_streams, cudaStream_t st);

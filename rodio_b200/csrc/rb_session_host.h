@@ -4,6 +4,7 @@
 // keeps running there; the CUDA build launches the kernels instead.  Same jobs, same order of the additions, one sample at a
 // time.  The translation unit is compiled with -ffp-contract=off, like the kernels.
 #pragma once
+#include <cmath>
 #include <limits>
 #include <utility>
 #include <vector>
@@ -111,6 +112,36 @@ cudaError_t rb_lanes_fifo_scatter_prog(const float* staging, const rb_fifo_prog_
                 if (!lanes::sample_in_class(v)) flags[j.row] = 1u;
                 fifo[(uint64_t)j.row * stride + ((uint64_t)j.fill + f) * j.ci + c] = v;
             }
+    }
+    return cudaSuccess;
+}
+
+// rb_dsp.cuh's generator (signal_phase_next, signal_value); the host's libm sinf is glibc's, which sinf_glibc_0_tau restates on
+// [0, 2*pi] (tests/test_signal_generator.py::test_sinf_restatement_against_libm)
+namespace session_host {
+inline float signal_value(uint32_t fn, float phase) {
+    switch (fn) {
+        case RB_SIGNAL_SINE: return sinf(6.2831855f * phase);
+        case RB_SIGNAL_TRIANGLE: return 4.0f * fabsf(phase - floorf(phase + 0.5f)) - 1.0f;
+        case RB_SIGNAL_SQUARE: return phase < 0.5f ? 1.0f : -1.0f;
+        default: return 2.0f * (phase - floorf(phase + 0.5f));
+    }
+}
+}  // namespace session_host
+
+cudaError_t rb_lanes_fifo_generate(const rb_fifo_gen_job* jobs, uint32_t n_jobs, const rb_prog_op* ops, const float* phase_in, float* phase_out,
+                                   float* fifo, uint64_t stride, uint32_t* flags, cudaStream_t) {
+    for (uint32_t k = 0; k < n_jobs; k++) {
+        const rb_fifo_gen_job& j = jobs[k];
+        float phase = phase_in[j.gen];
+        for (uint32_t f = 0; f < j.frames; f++) {
+            const float v = session_host::run_prog(session_host::signal_value(j.fn, phase), j.base + f, 1, ops + j.op0, j.n_ops);
+            if (!lanes::sample_in_class(v)) flags[j.row] = 1u;
+            fifo[(uint64_t)j.row * stride + j.fill + f] = v;
+            const float q = phase + j.step;
+            phase = j.step < 1.0f ? (q >= 1.0f ? q - 1.0f : q) : q - floorf(q);
+        }
+        phase_out[j.gen] = phase;
     }
     return cudaSuccess;
 }

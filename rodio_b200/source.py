@@ -337,10 +337,17 @@ class Function:
     Sine, Triangle, Square, Sawtooth = capi.RB_SIGNAL_SINE, capi.RB_SIGNAL_TRIANGLE, capi.RB_SIGNAL_SQUARE, capi.RB_SIGNAL_SAWTOOTH
 
 
+ENDLESS = 2**64 - 1     # ns[0] of RB_FX_SIGNAL: the generator never ends by itself
+
+
 class SignalGenerator:
     """source::SignalGenerator::new(sample_rate, frequency, function) -- src/source/signal_generator.rs:85-99: an endless mono
     source; `.take(n)` (Iterator::take, what the reference's tests and examples bound it with) gives the Source that is handed
-    to the mixer.  The samples are generated on the device (RB_FX_SIGNAL): nothing is uploaded."""
+    to the mixer.  The samples are generated on the device (RB_FX_SIGNAL): nothing is uploaded.
+    The Source adapters apply to the endless generator, as in rodio: `SineWave(740.0).amplify(0.1).take_duration(d)` -- a
+    streaming Session plays such a source until its take_duration ends it or Session.skip stops it."""
+
+    _ADAPTERS = frozenset(n for n in vars(Source) if not n.startswith("_") and n not in ("channels", "sample_rate", "collect"))
 
     def __init__(self, sample_rate: int, frequency: float, f: int = Function.Sine):
         if not float(np.float32(frequency)) > 0.0:
@@ -356,6 +363,15 @@ class SignalGenerator:
     def take(self, n: int) -> Source:
         e = Effect.make(capi.RB_FX_SIGNAL, u32=[self.function], f32=[self.frequency], ns=[int(n)])
         return Source(np.zeros(0, dtype=np.float32), 1, self.rate, 0, [e])
+
+    def endless(self) -> Source:
+        """The generator itself as a Source (ns[0] = ENDLESS)."""
+        return self.take(ENDLESS)
+
+    def __getattr__(self, name):
+        if name in SignalGenerator._ADAPTERS:
+            return getattr(self.endless(), name)
+        raise AttributeError(name)
 
 
 def SineWave(freq: float) -> SignalGenerator:
@@ -417,6 +433,8 @@ def UniformSourceIterator(input: Source, target_channels: int, target_sample_rat
     """source::UniformSourceIterator::new(input, channels, rate) — src/source/uniform.rs:33-47."""
     if target_channels <= 0 or target_sample_rate <= 0:
         raise ValueError("target channels / rate must be non-zero")
+    if isinstance(input, SignalGenerator):
+        input = input.endless()
     return input._with(Effect.make(capi.RB_FX_UNIFORM, u32=[target_channels, target_sample_rate]),
                        channels=target_channels, rate=target_sample_rate)
 
@@ -710,6 +728,8 @@ class Session:
         # mixer(channels, rate): the chains end in UniformSourceIterator(_, channels, rate), so they report the mixer's count
         self.channels = mixer_channels or (self.sources[0].channels() if self.sources else 1)
         self.src_channels = [s.base_channels for s in self.sources]       # what is pushed: the source's own interleaving
+        # generator sources (RB_FX_SIGNAL) fill themselves and take no pushes: the push helpers pass them by
+        self.generators = [bool(s.effects) and s.effects[0].kind == capi.RB_FX_SIGNAL for s in self.sources]
         self._descs, self._keep = pack_descs(self.sources, mix_starts)
         self._h = C.c_void_p()
         if restarts:
@@ -756,9 +776,13 @@ class Session:
     def push_packed(self, blocks: Sequence[np.ndarray], end_of_stream: Optional[Sequence[bool]] = None,
                     spans: Optional[Sequence[Sequence[Tuple[int, int]]]] = None):
         """One block per source (possibly empty), pushed with one copy and one kernel.  spans: one list of (at, span_len) marks per
-        source, as in push (rb_session_push_packed_spans)."""
+        source, as in push (rb_session_push_packed_spans).  The entries of generator sources are passed by."""
         assert len(blocks) == len(self.sources)
-        blocks = [np.ascontiguousarray(b, dtype=np.float32) for b in blocks]
+        blocks = [np.zeros(0, np.float32) if g else np.ascontiguousarray(b, dtype=np.float32) for b, g in zip(blocks, self.generators)]
+        if end_of_stream is not None:
+            end_of_stream = [bool(e) and not g for e, g in zip(end_of_stream, self.generators)]
+        if spans is not None:
+            spans = [() if g else sp for sp, g in zip(spans, self.generators)]
         flat = np.concatenate(blocks) if blocks else np.zeros(0, np.float32)
         n = (C.c_uint64 * len(blocks))(*[b.size // ch for b, ch in zip(blocks, self.src_channels)])
         eos = (C.c_uint8 * len(blocks))(*[int(bool(e)) for e in end_of_stream]) if end_of_stream is not None else None
